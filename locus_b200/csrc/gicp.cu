@@ -92,6 +92,10 @@ struct KTimer {          // CUDA-event timing of one kernel class
   uint64_t launches = 0;
 };
 
+// The per-device align budget (SmBudget below) counts half SMs: a CTA of the persistent and cluster kernels holds a
+// whole SM, a CTA of the 160-thread loop_solve_kernel half of one when two of them fit on an SM.
+constexpr int SM_SLOTS = 2;
+
 }  // namespace lb
 
 using namespace lb;
@@ -132,6 +136,7 @@ struct lb_gicp {
   OuterResult* d_result = nullptr; OuterResult* h_result = nullptr;
   LoopState* d_loop = nullptr; LoopState* h_loop = nullptr;    // stream-ordered execution: the outer loop's state
   int align_blocks = 0;
+  int wide_solve_slots = SM_SLOTS;   // budget slots one CTA of loop_solve_kernel<2 * AL_PPL, AL_SOLVE_THREADS> takes
   int knn_resident_blocks = 0;    // CTAs of knn_cov_quadreg_kernel that are resident at once on this device
   bool have_result = false;
   float final_T[16];
@@ -147,10 +152,11 @@ struct lb_gicp {
 
 namespace {
 
-// One align() kernel occupies its SMs exclusively (255 registers x 256 threads = the whole register file) and its
-// CTAs spin on each other, so the persistent kernels of concurrently used handles (lb_odometry workers, or a
-// caller's own threads) must fit on the device TOGETHER: more CTAs than SMs would leave a cooperative grid waiting
-// for SMs held by other spinning grids.  Per device, launches take their CTA count from this budget and give it
+// The CTAs of one align() kernel spin on each other, so the cooperative grids of concurrently used handles
+// (lb_odometry workers, or a caller's own threads) must fit on the device TOGETHER: more CTAs than fit would leave a
+// cooperative grid waiting for SMs held by other spinning grids.  A persistent or cluster CTA occupies a whole SM
+// (255 registers x 256 threads = the whole register file), and so does a 256-thread loop_solve_kernel CTA; a
+// 160-thread loop_solve_kernel CTA (168 registers) half of one.  Per device, launches take their share in half SMs (SM_SLOTS per SM) from this budget and give it
 // back after the stream sync; a few SMs stay reserved for the short kernels (VoxelGrid, index, k-NN) of the other
 // pipeline stages.  A lone align always runs.
 constexpr int LB_MAX_DEVICES = 64;
@@ -297,6 +303,18 @@ int gicp_create_impl(int device, void* stream, bool ext, lb_gicp** out) {
       return LB_ERR_CUDA;
     }
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, align_persistent_kernel<AL_PPL>, AL_THREADS, big);
+    // the stream-ordered solve at 8 points per lane: correspondences in dynamic shared memory, the carveout at its
+    // maximum so that two CTAs (2 x ~110 KB) fit on one SM
+    int solve_per_sm = 0;
+    const int solve_bytes = (int)SmemCacheT<2 * AL_PPL>::kBytes;
+    if (cudaFuncSetAttribute(loop_solve_kernel<2 * AL_PPL, AL_SOLVE_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, solve_bytes) != cudaSuccess ||
+        cudaFuncSetAttribute(loop_solve_kernel<2 * AL_PPL, AL_SOLVE_THREADS>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&solve_per_sm, loop_solve_kernel<2 * AL_PPL, AL_SOLVE_THREADS>, AL_SOLVE_THREADS, solve_bytes) != cudaSuccess) {
+      set_error("lb_gicp_create: solve kernel configuration refused: %s", cudaGetErrorString(cudaGetLastError()));
+      delete h;
+      return LB_ERR_CUDA;
+    }
+    h->wide_solve_slots = solve_per_sm >= SM_SLOTS ? 1 : SM_SLOTS;
   }
   {
     int knn_per_sm = 0;
@@ -1026,10 +1044,14 @@ int lb_gicp_align(lb_gicp* h, const float* guess_in, lb_gicp_result* out) {
     for (int i = 0; i < 16; i++) aa.guess[i] = guess[i];
     const int grid = grid_for(h, ca.n_src);
     static const int reserve_s = [] { const char* e = getenv("LB_SM_RESERVE"); return e ? atoi(e) : 16; }();
-    SmLease lease;
-    lease.acquire(c.device, grid, h->align_blocks - reserve_s);
     const int chunk = cdiv(ca.n_src, grid);
-    void* kfn = chunk <= AL_PPC ? (void*)loop_solve_kernel<AL_PPL> : (void*)loop_solve_kernel<2 * AL_PPL>;
+    // up to 512 points per CTA: the one-per-SM shape (lowest latency); beyond: the two-per-SM shape (throughput)
+    const bool wide = chunk > AL_PPC;
+    void* kfn = wide ? (void*)loop_solve_kernel<2 * AL_PPL, AL_SOLVE_THREADS> : (void*)loop_solve_kernel<AL_PPL, AL_THREADS>;
+    const int solve_threads = wide ? AL_SOLVE_THREADS : AL_THREADS;
+    const size_t solve_bytes = wide ? SmemCacheT<2 * AL_PPL>::kBytes : 0;
+    SmLease lease;
+    lease.acquire(c.device, grid * (wide ? h->wide_solve_slots : SM_SLOTS), SM_SLOTS * (h->align_blocks - reserve_s));
     {
       ScopedKernelTime kt(h, "align_persistent");
       for (int done = 0; !done;) {
@@ -1050,7 +1072,7 @@ int lb_gicp_align(lb_gicp* h, const float* guess_in, lb_gicp_result* out) {
           int kk = k;
           void* args[] = {&aa, &dl, &kk};
           ScopedKernelTime ks(h, "loop_solve");
-          LB_CUDA(cudaLaunchCooperativeKernel(kfn, dim3(grid), dim3(AL_THREADS), args, 0, c.stream));
+          LB_CUDA(cudaLaunchCooperativeKernel(kfn, dim3(grid), dim3(solve_threads), args, solve_bytes, c.stream));
           c.launches += 2;
         }
         LB_CUDA(cudaMemcpyAsync(h->h_loop, h->d_loop, sizeof(LoopState), cudaMemcpyDeviceToHost, c.stream));
@@ -1102,7 +1124,7 @@ int lb_gicp_align(lb_gicp* h, const float* guess_in, lb_gicp_result* out) {
       cfg.attrs = at; cfg.numAttrs = 2;
       // the solver cluster and its helpers spin on each other like the all-SM grid does: same per-device SM budget
       static const int reserve_c = [] { const char* ev = getenv("LB_SM_RESERVE"); return ev ? atoi(ev) : 16; }();
-      lease.acquire(c.device, CL_SIZE * clusters, h->align_blocks - reserve_c);
+      lease.acquire(c.device, SM_SLOTS * CL_SIZE * clusters, SM_SLOTS * (h->align_blocks - reserve_c));
       ScopedKernelTime kt(h, "align_persistent");
       cudaError_t e = cudaLaunchKernelEx(&cfg, align_cluster_kernel, ka);
       if (e == cudaSuccess) { launched = true; c.launches++; }
@@ -1120,7 +1142,7 @@ int lb_gicp_align(lb_gicp* h, const float* guess_in, lb_gicp_result* out) {
       void* args[] = {&aa};
       const int grid = grid_for(h, ca.n_src);
       static const int reserve = [] { const char* e = getenv("LB_SM_RESERVE"); return e ? atoi(e) : 16; }();
-      lease.acquire(c.device, grid, h->align_blocks - reserve);
+      lease.acquire(c.device, SM_SLOTS * grid, SM_SLOTS * (h->align_blocks - reserve));
       ScopedKernelTime kt(h, "align_persistent");
       // points per CTA up to 512: 4 per accumulating lane in registers; up to 1024: 8 (beyond: read back from L2)
       const int chunk = cdiv(ca.n_src, grid);

@@ -13,6 +13,8 @@
 //   transform_kernel, nn_query_kernel, fitness_kernel   accessor surface (a8/a9)
 #pragma once
 
+#include <type_traits>
+
 #include "bfgs.h"
 #include "grid.h"
 #include "nn_staged.cuh"
@@ -30,6 +32,11 @@ constexpr int AL_PPC = AL_ACC * 4;   // source points per CTA (4 per accumulatin
 constexpr int AL_MAXV = 28;          // widest reduction (Gauss-Newton)
 constexpr int AL_PSTRIDE = 32;       // words per CTA slot
 constexpr int AL_MAXB = 8;           // slots per polling lane: supports up to 256 CTAs
+// loop_solve_kernel runs no correspondence search, so its CTA can be the leader warp and the accumulating warps only:
+// 160 threads at <= 168 registers (registers are allocated per SM sub-partition: 3 warps of 168 fit in one of the
+// four, 2 of 200), two CTAs per SM
+constexpr int AL_SOLVE_THREADS = 32 + AL_ACC;
+constexpr int AL_SOLVE_POLL = 8;     // slot words one thread of the solve kernel polls at a time
 
 // ------------------------------------------------------------------ cloud upload
 __global__ void __launch_bounds__(256)
@@ -953,48 +960,52 @@ __device__ __forceinline__ bool slot_try(const SlotWord* p, unsigned long long e
 // Every (slot, value) pair is polled by exactly one thread of the CTA, all pairs in flight at once (one L2
 // round trip when nobody is late); the values land in a shared matrix and warp w then sums rows e = w,
 // w + nwarps, ... lane-strided + shuffle tree.  out[e] (shared) valid after the trailing CTA barrier.
+// A thread holds at most CHUNK words in registers: with fewer than all of its pairs (the solve kernel's register
+// budget), the pairs are gathered CHUNK per thread at a time, one after the other.
 constexpr int AL_MAXCTA = 160;
 constexpr long long AL_POLL_DELAY = 400;   // cycles before the first poll; chosen on an earlier GPU, not re-tuned for the H100
-template <int NV, int THREADS>
+template <int NV, int THREADS, int CHUNK = (AL_MAXCTA * NV + THREADS - 1) / THREADS>
 __device__ __forceinline__ void slots_all_sum(const SlotWord* buf, int ncta, unsigned long long epoch,
                                               double* mat /*[NV][AL_MAXCTA] shared*/, double* out /*shared [NV]*/,
                                               long long* prof_rounds = nullptr, long long poll_delay = AL_POLL_DELAY) {
+  static_assert(CHUNK >= 1 && CHUNK <= 32, "one bit of the pending mask per word in flight");
   const int npairs = ncta * NV;
-  constexpr int MAXP = (AL_MAXCTA * NV + THREADS - 1) / THREADS;
   // every CTA publishes at about the same time and a publication takes a while to land in L2: polling at once
   // wastes a full round trip on words that are not there yet, so hold the first poll back a little
   {
     const long long t_start = clock64();
     while (clock64() - t_start < poll_delay) {}
   }
-  unsigned pending = 0;
-#pragma unroll
-  for (int k = 0; k < MAXP; k++)
-    if ((int)threadIdx.x + k * THREADS < npairs) pending |= 1u << k;
   int rounds = 0;
-  while (pending) {
-    rounds++;
-    // issue every pending load first, then look at the tags: the loads of one round overlap (one L2 round trip)
-    unsigned long long lo[MAXP], hi[MAXP];
+  for (int first = 0; first < npairs; first += CHUNK * THREADS) {
+    unsigned pending = 0;
 #pragma unroll
-    for (int k = 0; k < MAXP; k++) {
-      lo[k] = 0; hi[k] = 0;
-      if (pending & (1u << k)) {
-        int pr = threadIdx.x + k * THREADS;
-        int b = pr / NV, e = pr - b * NV;
-        const SlotWord* p = &buf[(size_t)b * AL_PSTRIDE + e];
-        asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(lo[k]), "=l"(hi[k]) : "l"(p));
+    for (int k = 0; k < CHUNK; k++)
+      if (first + (int)threadIdx.x + k * THREADS < npairs) pending |= 1u << k;
+    while (pending) {
+      rounds++;
+      // issue every pending load first, then look at the tags: the loads of one round overlap (one L2 round trip)
+      unsigned long long lo[CHUNK], hi[CHUNK];
+#pragma unroll
+      for (int k = 0; k < CHUNK; k++) {
+        lo[k] = 0; hi[k] = 0;
+        if (pending & (1u << k)) {
+          int pr = first + threadIdx.x + k * THREADS;
+          int b = pr / NV, e = pr - b * NV;
+          const SlotWord* p = &buf[(size_t)b * AL_PSTRIDE + e];
+          asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(lo[k]), "=l"(hi[k]) : "l"(p));
+        }
       }
+      const unsigned long long tag = epoch & 0xffffffffull;
+#pragma unroll
+      for (int k = 0; k < CHUNK; k++)
+        if ((pending & (1u << k)) && (lo[k] >> 32) == tag && (hi[k] >> 32) == tag) {
+          int pr = first + threadIdx.x + k * THREADS;
+          int b = pr / NV, e = pr - b * NV;
+          mat[e * AL_MAXCTA + b] = __longlong_as_double((long long)((hi[k] << 32) | (lo[k] & 0xffffffffull)));
+          pending &= ~(1u << k);
+        }
     }
-    const unsigned long long tag = epoch & 0xffffffffull;
-#pragma unroll
-    for (int k = 0; k < MAXP; k++)
-      if ((pending & (1u << k)) && (lo[k] >> 32) == tag && (hi[k] >> 32) == tag) {
-        int pr = threadIdx.x + k * THREADS;
-        int b = pr / NV, e = pr - b * NV;
-        mat[e * AL_MAXCTA + b] = __longlong_as_double((long long)((hi[k] << 32) | (lo[k] & 0xffffffffull)));
-        pending &= ~(1u << k);
-      }
   }
   if (prof_rounds) { prof_rounds[0] += rounds; prof_rounds[1] += clock64(); }
   __syncthreads();
@@ -1270,27 +1281,68 @@ __device__ __forceinline__ int acc_lane() { return (int)threadIdx.x - 32 * AL_AC
 // (the correspondences are fixed during the inner solve, gicp.hpp:518-524): zero memory traffic per evaluation.
 template <int PPL>
 struct PointCacheT {
+  static constexpr int kPPL = PPL;
   float px[PPL], py[PPL], pz[PPL], qx[PPL], qy[PPL], qz[PPL];
   double M[PPL][6];
 };
 using PointCache = PointCacheT<AL_PPL>;
+
+// The same correspondences in dynamic shared memory, for loop_solve_kernel: registers held for the whole solve would
+// not leave room for two CTAs per SM.  Lane-fastest ([field][point][lane]): a warp's accesses are conflict-free.
+// The accessors address the dynamic shared array directly (no pointer members): the compiler then emits shared-window
+// loads with immediate offsets instead of keeping 64-bit generic addresses live.
+extern __shared__ __align__(16) unsigned char al_cache_smem[];
+template <int PPL>
+struct SmemCacheT {
+  static constexpr int kPPL = PPL;
+  static constexpr size_t kBytes = (size_t)6 * PPL * AL_ACC * (sizeof(double) + sizeof(float));
+  // M: [6][PPL][AL_ACC] doubles, then [6][PPL][AL_ACC] floats px, py, pz, qx, qy, qz
+  __device__ __forceinline__ double& m(int e, int j, int t) const {
+    return reinterpret_cast<double*>(al_cache_smem)[(e * PPL + j) * AL_ACC + t];
+  }
+  __device__ __forceinline__ float& f(int c, int j, int t) const {
+    return reinterpret_cast<float*>(al_cache_smem + (size_t)6 * PPL * AL_ACC * sizeof(double))[(c * PPL + j) * AL_ACC + t];
+  }
+};
+
+// point j of accumulating lane t of the chunk [begin, end): source point p, matched point c, M.  Points past the end
+// and unmatched points come back as zeros, whose M = 0 adds exact zeros.
+__device__ __forceinline__ void cache_fetch(const ObjArgs& a, int begin, int end, int t, int j, f4& p, f4& c, double* M) {
+  int s = begin + t + AL_ACC * j;
+  bool ok = (t >= 0 && t < AL_ACC && s < end);
+  // corr / M may have been written by a warp of another SM (far queue of the staged search): read them from L2
+  c = f4{0.f, 0.f, 0.f, bits_to_float(-1)};
+  if (ok) { const float4 cc = __ldcg(reinterpret_cast<const float4*>(a.corr + s)); c = f4{cc.x, cc.y, cc.z, cc.w}; }
+  ok = ok && float_to_bits(c.w) >= 0;
+  p = ok ? a.src[s] : f4{0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int e = 0; e < 6; e++) M[e] = ok ? __ldcg(a.M + 6 * (size_t)s + e) : 0.0;
+}
 
 template <int PPL>
 __device__ __forceinline__ void cache_load(const ObjArgs& a, int begin, int end, PointCacheT<PPL>& pc) {
   const int t = acc_lane();
 #pragma unroll
   for (int j = 0; j < PPL; j++) {
-    int s = begin + t + AL_ACC * j;
-    bool ok = (t >= 0 && t < AL_ACC && s < end);
-    // corr / M may have been written by a warp of another SM (far queue of the staged search): read them from L2
-    f4 c = f4{0.f, 0.f, 0.f, bits_to_float(-1)};
-    if (ok) { const float4 cc = __ldcg(reinterpret_cast<const float4*>(a.corr + s)); c = f4{cc.x, cc.y, cc.z, cc.w}; }
-    ok = ok && float_to_bits(c.w) >= 0;
-    f4 p = ok ? a.src[s] : f4{0.f, 0.f, 0.f, 0.f};
+    f4 p, c;
+    cache_fetch(a, begin, end, t, j, p, c, pc.M[j]);
     pc.px[j] = p.x; pc.py[j] = p.y; pc.pz[j] = p.z;
     pc.qx[j] = c.x; pc.qy[j] = c.y; pc.qz[j] = c.z;
+  }
+}
+
+template <int PPL>
+__device__ __forceinline__ void cache_load(const ObjArgs& a, int begin, int end, SmemCacheT<PPL>& pc) {
+  const int t = acc_lane();
 #pragma unroll
-    for (int e = 0; e < 6; e++) pc.M[j][e] = ok ? __ldcg(a.M + 6 * (size_t)s + e) : 0.0;   // M = 0: exact zero contribution
+  for (int j = 0; j < PPL; j++) {
+    f4 p, c;
+    double M[6];
+    cache_fetch(a, begin, end, t, j, p, c, M);
+    pc.f(0, j, t) = p.x; pc.f(1, j, t) = p.y; pc.f(2, j, t) = p.z;
+    pc.f(3, j, t) = c.x; pc.f(4, j, t) = c.y; pc.f(5, j, t) = c.z;
+#pragma unroll
+    for (int e = 0; e < 6; e++) pc.m(e, j, t) = M[e];
   }
 }
 
@@ -1301,6 +1353,22 @@ __device__ __forceinline__ void objective_from_cache(const PointCacheT<PPL>& pc,
   for (int j = 0; j < PPL; j++) {
     if constexpr (NV == 13) objective_terms(T, pc.px[j], pc.py[j], pc.pz[j], pc.qx[j], pc.qy[j], pc.qz[j], pc.M[j], acc);
     else gn_terms(T, dP, dT, dS, pc.px[j], pc.py[j], pc.pz[j], pc.qx[j], pc.qy[j], pc.qz[j], pc.M[j], acc);
+  }
+}
+
+template <int NV, int PPL>
+__device__ __forceinline__ void objective_from_cache(const SmemCacheT<PPL>& pc, const float* T, const double* dP, const double* dT,
+                                                     const double* dS, double* acc) {
+  const int t = acc_lane();
+#pragma unroll 1
+  for (int j = 0; j < PPL; j++) {
+    double M[6];
+#pragma unroll
+    for (int e = 0; e < 6; e++) M[e] = pc.m(e, j, t);
+    const float px = pc.f(0, j, t), py = pc.f(1, j, t), pz = pc.f(2, j, t);
+    const float qx = pc.f(3, j, t), qy = pc.f(4, j, t), qz = pc.f(5, j, t);
+    if constexpr (NV == 13) objective_terms(T, px, py, pz, qx, qy, qz, M, acc);
+    else gn_terms(T, dP, dT, dS, px, py, pz, qx, qy, qz, M, acc);
   }
 }
 
@@ -1423,9 +1491,11 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 }
 
 // grid-wide deterministic sum of the NV doubles held by the accumulating lanes; totals land in
-// sh.bc[0..NV-1] (visible to all threads after return)
-template <int NV>
+// sh.bc[0..NV-1] (visible to all threads after return).  THREADS: the CTA size of the calling kernel.
+template <int NV, int THREADS>
 __device__ __forceinline__ void grid_all_reduce(const AlignArgs& a, AlignShared& sh, Collective& co, double* acc) {
+  constexpr int all_pairs = (AL_MAXCTA * NV + THREADS - 1) / THREADS;
+  constexpr int chunk = THREADS == AL_THREADS ? all_pairs : (all_pairs < AL_SOLVE_POLL ? all_pairs : AL_SOLVE_POLL);
   const bool prof = (blockIdx.x == 0 && threadIdx.x == 0);
   long long t0 = prof ? clock64() : 0;
   double tot = block_reduce<NV, AL_ACC_WARPS, AL_ACC_W0>(acc, sh.red);
@@ -1436,13 +1506,14 @@ __device__ __forceinline__ void grid_all_reduce(const AlignArgs& a, AlignShared&
   long long t1 = prof ? clock64() : 0;
   const bool snap = a.debug && threadIdx.x == 0 && (co.epoch - a.epoch_base) == 100;   // one collective, all CTAs
   if (snap) a.debug[16 + blockIdx.x] = (long long)globaltimer_ns();
-  slots_all_sum<NV, AL_THREADS>(buf, ncta, co.epoch, sh.mat, sh.bc, prof ? sh.poll : nullptr, (long long)a.poll_delay);
+  slots_all_sum<NV, THREADS, chunk>(buf, ncta, co.epoch, sh.mat, sh.bc, prof ? sh.poll : nullptr, (long long)a.poll_delay);
   if (prof) sh.poll[1] -= t1;   // accumulates (poll completion - publish) for thread 0
   if (snap) a.debug[16 + AL_MAXCTA + blockIdx.x] = (long long)globaltimer_ns();
   co.flip ^= 1;
   if (prof) { long long t2 = clock64(); sh.t_reduce += t1 - t0; sh.t_wait += t2 - t1; sh.n_coll++; sh.t_mark = t2; }
 }
 
+// (the persistent kernel only: its 256-thread CTA runs the search)
 template <int PPL>
 __device__ __forceinline__ void do_correspond(const AlignArgs& a, AlignShared& sh, Collective& co, PointCacheT<PPL>& pc) {
   float T[12]; double R[9];
@@ -1466,7 +1537,7 @@ __device__ __forceinline__ void do_correspond(const AlignArgs& a, AlignShared& s
     // grid takes its share of them
     __threadfence();
     double zero[1] = {0.0};
-    grid_all_reduce<1>(a, sh, co, zero);
+    grid_all_reduce<1, AL_THREADS>(a, sh, co, zero);
     const int nfar = *(volatile int*)(a.c.far_count + (calls & 1));
     if (blockIdx.x == 0 && threadIdx.x == 0) a.c.far_count[(calls & 1) ^ 1] = 0;      // the next step's counter
     hits += correspond_far(a.c, T, R, nfar, (int)blockIdx.x * (AL_THREADS / 32) + (int)(threadIdx.x >> 5),
@@ -1488,7 +1559,7 @@ __device__ __forceinline__ void do_correspond(const AlignArgs& a, AlignShared& s
     cnt[0] = (double)h;
   }
   const long long q1 = cprof ? clock64() : 0;
-  grid_all_reduce<1>(a, sh, co, cnt);
+  grid_all_reduce<1, AL_THREADS>(a, sh, co, cnt);
   if (end - begin <= PPL * AL_ACC && t >= 0 && t < AL_ACC) {
     ObjArgs oa{a.c.src, a.c.corr, a.c.M, a.c.n_src};
     cache_load<PPL>(oa, begin, end, pc);
@@ -1496,8 +1567,10 @@ __device__ __forceinline__ void do_correspond(const AlignArgs& a, AlignShared& s
   if (cprof) { a.debug[14] += q1 - q0; a.debug[15] += clock64() - q1; }
 }
 
-template <int NV, int PPL>
-__device__ __forceinline__ void do_objective(const AlignArgs& a, AlignShared& sh, Collective& co, const PointCacheT<PPL>& pc) {
+// Cache: PointCacheT (registers) or SmemCacheT (shared memory); THREADS: the CTA size of the calling kernel
+template <int NV, int THREADS, class Cache>
+__device__ __forceinline__ void do_objective(const AlignArgs& a, AlignShared& sh, Collective& co, const Cache& pc) {
+  constexpr int PPL = Cache::kPPL;
   float T[12];
 #pragma unroll
   for (int i = 0; i < 12; i++) T[i] = sh.T[i];
@@ -1513,19 +1586,20 @@ __device__ __forceinline__ void do_objective(const AlignArgs& a, AlignShared& sh
     ObjArgs oa{a.c.src, a.c.corr, a.c.M, a.c.n_src};
     objective_from_global<NV>(oa, T, sh.D, sh.D + 9, sh.D + 18, begin, end, acc);
   }
-  grid_all_reduce<NV>(a, sh, co, acc);
+  grid_all_reduce<NV, THREADS>(a, sh, co, acc);
 }
 
 // Backend of bfgs.h for the leader warp (all 32 lanes call every method together).
-template <int PPL>
+template <class Cache, int THREADS>
 struct DeviceBackendT {
+  static constexpr int PPL = Cache::kPPL;
   const AlignArgs& a;
   AlignShared& sh;
   Collective& co;
-  PointCacheT<PPL>& pc;     // warp 0 never accumulates: its cache is never read
+  Cache& pc;     // warp 0 never accumulates: its cache is never read
   int m;
 
-  __device__ DeviceBackendT(const AlignArgs& a_, AlignShared& sh_, Collective& co_, PointCacheT<PPL>& pc_)
+  __device__ DeviceBackendT(const AlignArgs& a_, AlignShared& sh_, Collective& co_, Cache& pc_)
       : a(a_), sh(sh_), co(co_), pc(pc_), m(0) {}
 
   // the 12 trigonometric values of a state, one per lane, broadcast to the warp
@@ -1570,7 +1644,7 @@ struct DeviceBackendT {
     if (lane == 0) sh.op = OP_FDF;
     if (blockIdx.x == 0 && threadIdx.x == 0) sh.t_scalar += clock64() - sh.t_mark;   // leader time since the last collective
     __syncthreads();
-    do_objective<13, PPL>(a, sh, co, pc);
+    do_objective<13, THREADS>(a, sh, co, pc);
     double sums[13];
 #pragma unroll
     for (int e = 0; e < 13; e++) sums[e] = sh.bc[e];
@@ -1589,7 +1663,7 @@ struct DeviceBackendT {
     if (lane < 27) sh.D[lane] = D[lane];
     if (lane == 0) sh.op = OP_GN;
     __syncthreads();
-    do_objective<28, PPL>(a, sh, co, pc);
+    do_objective<28, THREADS>(a, sh, co, pc);
     *f = sh.bc[0] / (double)m;
 #pragma unroll
     for (int e = 0; e < 6; e++) b[e] = sh.bc[1 + e];
@@ -1617,7 +1691,7 @@ align_persistent_kernel(const __grid_constant__ AlignArgs a) {
   if (a.c.nn_mode) { NnsCta nc{nns_dyn_smem, a.c.nn_cap}; NnsWarp w0 = nns_warp_view(nc); nns_warp_init(w0); }
   if (threadIdx.x < 32) {
     PointCacheT<PPL> pc_unused;   // warp 0 does not accumulate; kept apart from the workers' register-resident cache
-    DeviceBackendT<PPL> be(a, sh, co, pc_unused);
+    DeviceBackendT<PointCacheT<PPL>, AL_THREADS> be(a, sh, co, pc_unused);
     OuterResult r;
     gicp_outer_loop(be, a.P, a.guess, r);
     if (threadIdx.x == 0) sh.op = OP_EXIT;
@@ -1636,8 +1710,8 @@ align_persistent_kernel(const __grid_constant__ AlignArgs a) {
       const int op = sh.op;
       if (op == OP_EXIT) break;
       if (op == OP_CORR) do_correspond<PPL>(a, sh, co, pc);
-      else if (op == OP_FDF) do_objective<13, PPL>(a, sh, co, pc);
-      else do_objective<28, PPL>(a, sh, co, pc);
+      else if (op == OP_FDF) do_objective<13, AL_THREADS>(a, sh, co, pc);
+      else do_objective<28, AL_THREADS>(a, sh, co, pc);
     }
   }
 }
@@ -1694,21 +1768,29 @@ loop_far_kernel(CorrArgs a, LoopState* __restrict__ st, int k) {
   if ((threadIdx.x & 31) == 0 && hits) atomicAdd(&st->m[k], hits);
 }
 
-template <int PPL>
-__global__ void __launch_bounds__(AL_THREADS, AL_MINB)
+// Two shapes, chosen by the host from the points per CTA:
+//   THREADS = AL_THREADS (4 points per lane: the lowest latency of one align): the persistent kernel's CTA, one per SM,
+//     255 registers, correspondences in registers (PointCacheT);
+//   THREADS = AL_SOLVE_THREADS (8 points per lane: the odometry pipeline's workers): the leader warp and the
+//     accumulating warps only, 168 registers, correspondences in dynamic shared memory (SmemCacheT<PPL>::kBytes per
+//     CTA), two CTAs per SM -- twice the aligns in flight under the per-device budget.
+// Same reduction shape and summation order in both: identical bits.
+template <int PPL, int THREADS>
+__global__ void __launch_bounds__(THREADS, THREADS == AL_SOLVE_THREADS ? 2 : AL_MINB)
 loop_solve_kernel(const __grid_constant__ AlignArgs a, LoopState* __restrict__ st, int k) {
+  using Cache = typename std::conditional<THREADS == AL_SOLVE_THREADS, SmemCacheT<PPL>, PointCacheT<PPL>>::type;
   __shared__ AlignShared sh;
-  if (st->s.done) return;                       // converged in an earlier launch of this batch (uniform for the grid)
+  if (st->s.done) return;                      // converged in an earlier launch of this batch (uniform for the grid)
   Collective co;
   co.epoch = a.epoch_base; co.flip = 0;
   if (threadIdx.x == 0) { sh.t_reduce = 0; sh.t_wait = 0; sh.n_coll = 0; sh.t_scalar = 0; sh.t_corr = 0; sh.t_mark = clock64(); sh.poll[0] = 0; sh.poll[1] = 0; }
   if (threadIdx.x < 32) {
-    PointCacheT<PPL> pc_unused;
-    DeviceBackendT<PPL> be(a, sh, co, pc_unused);
+    Cache pc_unused;
+    DeviceBackendT<Cache, THREADS> be(a, sh, co, pc_unused);
     OuterState s = st->s;
     const int m = st->m[k];
     be.m = m;
-    if (threadIdx.x == 0) sh.op = OP_LOAD;      // workers: this CTA's correspondences -> registers
+    if (threadIdx.x == 0) sh.op = OP_LOAD;      // workers: this CTA's correspondences -> the cache
     __syncthreads();
     outer_step(s, be, a.P, m);
     if (threadIdx.x == 0) sh.op = OP_EXIT;
@@ -1728,7 +1810,7 @@ loop_solve_kernel(const __grid_constant__ AlignArgs a, LoopState* __restrict__ s
       st->s = s;
     }
   } else {
-    PointCacheT<PPL> pc;
+    Cache pc;
     for (;;) {
       __syncthreads();
       const int op = sh.op;
@@ -1742,8 +1824,8 @@ loop_solve_kernel(const __grid_constant__ AlignArgs a, LoopState* __restrict__ s
           cache_load<PPL>(oa, begin, end, pc);
         }
       }
-      else if (op == OP_FDF) do_objective<13, PPL>(a, sh, co, pc);
-      else do_objective<28, PPL>(a, sh, co, pc);
+      else if (op == OP_FDF) do_objective<13, THREADS>(a, sh, co, pc);
+      else do_objective<28, THREADS>(a, sh, co, pc);
     }
   }
 }
