@@ -40,6 +40,10 @@
  *                                 point_cloud_filter/src/normal_computation.cc:26-59
  *   lb_gicp_compute_normals_radius   the same nodelet in its radius mode + removeNaNNormalsFromPointCloud
  *                                 normal_computation.cc:53-57,73-77
+ *   lb_gicp_statistical_outlier_removal   pcl::StatisticalOutlierRemoval<PointF>  point_cloud_filter/src/
+ *                                 PointCloudFilter.cc:126-133 (filtering/outlier_filter, run from locus/src/Locus.cc:450)
+ *   lb_gicp_radius_outlier_removal   pcl::RadiusOutlierRemoval<PointF>  PointCloudFilter.cc:135-143 and
+ *                                 point_cloud_merger/src/PointCloudMerger.cc:112-117,139-144,169-174
  *   lb_voxel_create/destroy       pcl::VoxelGrid<pcl::PCLPointCloud2> impl_
  *                                 point_cloud_filter/include/point_cloud_filter/custom_voxel_grid.h:25
  *   lb_voxel_set_leaf_size        impl_.setLeafSize()      custom_voxel_grid.cc:62-73, 97-101
@@ -240,6 +244,31 @@ int lb_gicp_compute_normals(lb_gicp* h, int which, int k, const float* viewpoint
  * exceeds 2048 points. */
 int lb_gicp_compute_normals_radius(lb_gicp* h, int which, double radius, const float* viewpoint, float* out4,
                                    int32_t* valid_idx, size_t* n_valid, int mem);
+/* SURVEY 8f row f5 -- the outlier filters of point_cloud_filter (PointCloudFilter.cc:126-143) and point_cloud_merger
+ * (PointCloudMerger.cc:112-117,139-144,169-174), i.e. pcl::StatisticalOutlierRemoval / pcl::RadiusOutlierRemoval
+ * (applyFilterIndices of filters/impl/statistical_outlier_removal.hpp and radius_outlier_removal.hpp, PCL 1.10), on the cloud currently set as source (which = 0)
+ * or target (which = 1).  Those clouds are dense (lb_gicp_set_source refuses non-finite points).  Output: kept_idx
+ * (capacity n) = ascending indices of the points the filter keeps, PCL's output order; *n_kept = their number.  All
+ * buffers host or all device (`mem`).  The handle's clouds, index and covariances stay as they were.
+ *
+ * Statistical: per point the mean_k + 1 nearest neighbours (itself included, ascending (d2, index));
+ *   distance = (float)(sum of sqrtf(d2) over neighbours 1..mean_k, in double, / mean_k).  sqrtf is the pinned reading of
+ *   PCL's unqualified sqrt on a float.  Then, serially in input order, sum += distance and sq_sum += distance * distance
+ *   (a float product) in double; mean = sum / n, variance = (sq_sum - sum * sum / n) / (n - 1), stddev = sqrt(variance),
+ *   threshold = mean + std_mul * stddev.  Removed iff distance > threshold (negative: distance <= threshold).  A NaN
+ *   threshold removes nothing (PCL's n == 1 case, which mean_k >= 1 already refuses).  mean_dist (nullable): n floats,
+ *   the per-point distance; stats3 (nullable): {mean, stddev, threshold}.  1 <= mean_k <= 19 (LB_ERR_UNSUPPORTED above);
+ *   n < mean_k + 1 -> LB_ERR_TOO_FEW_POINTS.
+ * Radius: `dense` selects PCL's branch on input->is_dense.  dense = 1: nearestKSearch(min_neighbors + 1), inlier iff that
+ *   many points came back and !(r^2 (double) < d2 of the last) -- i.e. at least min_neighbors + 1 points with
+ *   (double)d2 <= r^2.  dense = 0: radiusSearch, inlier iff more than min_neighbors points have d2 < float(r^2)
+ *   (FLANN's strict compare).  Both count the point itself.  negative keeps the outliers instead.  radius <= 0 ->
+ *   LB_ERR_INVALID_ARG (PCL logs an error and outputs nothing for radius 0).  min_neighbors = 0 keeps every point
+ *   (with dense = 0, as long as float(r^2) > 0). */
+int lb_gicp_statistical_outlier_removal(lb_gicp* h, int which, int mean_k, double std_mul, int negative,
+                                        int32_t* kept_idx, size_t* n_kept, float* mean_dist, double* stats3, int mem);
+int lb_gicp_radius_outlier_removal(lb_gicp* h, int which, double radius, int min_neighbors, int dense, int negative,
+                                   int32_t* kept_idx, size_t* n_kept, int mem);
 /* covariances used by the last align, n x 9 doubles row-major, original point order. which: 0 source, 1 target */
 int lb_gicp_get_covariances(lb_gicp* h, int which, double* out9, size_t capacity_points);
 /* number of points currently indexed. which: 0 source, 1 target */
@@ -305,7 +334,8 @@ int lb_voxel_filter(lb_voxel* h, const uint8_t* data, size_t n_pts, uint32_t poi
  *   output (pcl_ros::transformPointCloud: Eigen Matrix4f * Vector4f per point).  Then, on the transformed
  *   coordinates: the BodyFilter box, the VoxelGrid limits and the grid itself, exactly as lb_voxel_filter.  Needs the
  *   x, y, z, intensity layout (four averaged FLOAT32 fields) when more than one input or a transform is given.
- *   The merger's optional random / radius-outlier filters (off in the shipped config) are not part of this call. */
+ *   The merger's optional filters (off in the shipped config) are not part of this call: its radius-outlier filter is
+ *   lb_gicp_radius_outlier_removal on the merged cloud; its random sampler (seeded with time(nullptr)) has no GPU form. */
 typedef struct lb_voxel_input {
   const uint8_t* data;        /* n_pts points of point_step bytes (host or device: mem_in) */
   size_t n_pts;

@@ -89,7 +89,8 @@ SYMBOLS = [
     "lb_gicp_set_params", "lb_gicp_get_params", "lb_gicp_set_source", "lb_gicp_set_target",
     "lb_gicp_promote_source_to_target", "lb_gicp_reserve", "lb_gicp_prepare_source", "lb_gicp_share_source", "lb_gicp_set_target_cloud",
     "lb_cloud_release", "lb_gicp_align", "lb_gicp_transform_source", "lb_gicp_nn_target",
-    "lb_gicp_fitness", "lb_gicp_point2plane_information", "lb_gicp_compute_normals", "lb_gicp_compute_normals_radius", "lb_gicp_get_covariances", "lb_gicp_cloud_size", "lb_gicp_launch_count",
+    "lb_gicp_fitness", "lb_gicp_point2plane_information", "lb_gicp_compute_normals", "lb_gicp_compute_normals_radius",
+    "lb_gicp_statistical_outlier_removal", "lb_gicp_radius_outlier_removal", "lb_gicp_get_covariances", "lb_gicp_cloud_size", "lb_gicp_launch_count",
     "lb_gicp_kernel_time", "lb_gicp_reset_kernel_times",
     "lb_voxel_create", "lb_voxel_create_on_stream", "lb_voxel_destroy", "lb_voxel_set_leaf_size",
     "lb_voxel_get_leaf_size", "lb_voxel_set_filter_limits", "lb_voxel_set_min_points_per_voxel",
@@ -163,6 +164,9 @@ def lib():
         L.lb_gicp_compute_normals.argtypes = [vp, i32, i32, vp, vp, i32]
     if hasattr(L, "lb_gicp_compute_normals_radius"):
         L.lb_gicp_compute_normals_radius.argtypes = [vp, i32, C.c_double, vp, vp, vp, C.POINTER(sz), i32]
+    if hasattr(L, "lb_gicp_statistical_outlier_removal"):
+        L.lb_gicp_statistical_outlier_removal.argtypes = [vp, i32, i32, C.c_double, i32, vp, C.POINTER(sz), vp, vp, i32]
+        L.lb_gicp_radius_outlier_removal.argtypes = [vp, i32, C.c_double, i32, i32, i32, vp, C.POINTER(sz), i32]
     L.lb_gicp_cloud_size.argtypes = [vp, i32, C.POINTER(sz)]
     L.lb_gicp_launch_count.argtypes = [vp, u64p]
     L.lb_gicp_kernel_time.argtypes = [vp, C.c_char_p, C.POINTER(C.c_float), u64p]
@@ -443,6 +447,26 @@ class GicpB200:
         vp_ = None if viewpoint is None else np.ascontiguousarray(viewpoint, dtype=np.float32)
         _check(lib().lb_gicp_compute_normals_radius(self._h, which, float(radius), _ptr(vp_), _ptr(out), _ptr(vi), C.byref(m), LB_MEM_HOST))
         return out, vi[: m.value]
+
+    def statisticalOutlierRemoval(self, which=0, mean_k=10, std_mul=1.0, negative=False):
+        """pcl::StatisticalOutlierRemoval on the source (which=0) or target (which=1) cloud: (kept indices int32
+        ascending, per-point mean distance (n,) float32, [mean, stddev, threshold] float64)"""
+        n = self.cloudSize(which)
+        kept = np.zeros(max(n, 1), dtype=np.int32); md = np.zeros(n, dtype=np.float32); st = np.zeros(3)
+        m = C.c_size_t(0)
+        _check(lib().lb_gicp_statistical_outlier_removal(self._h, which, int(mean_k), float(std_mul), int(bool(negative)),
+                                                         _ptr(kept), C.byref(m), _ptr(md), _ptr(st), LB_MEM_HOST))
+        return kept[: m.value], md, st
+
+    def radiusOutlierRemoval(self, which=0, radius=0.15, min_neighbors=3, dense=True, negative=False):
+        """pcl::RadiusOutlierRemoval on the source (which=0) or target (which=1) cloud; dense = the input's is_dense
+        (PCL's k-NN branch) or not (its radius-search branch).  Returns the kept indices, int32 ascending."""
+        n = self.cloudSize(which)
+        kept = np.zeros(max(n, 1), dtype=np.int32)
+        m = C.c_size_t(0)
+        _check(lib().lb_gicp_radius_outlier_removal(self._h, which, float(radius), int(min_neighbors), int(bool(dense)),
+                                                    int(bool(negative)), _ptr(kept), C.byref(m), LB_MEM_HOST))
+        return kept[: m.value]
 
     def launchCount(self):
         n = C.c_uint64(0)

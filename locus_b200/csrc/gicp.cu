@@ -229,6 +229,13 @@ float float_gate(double D) {
   return g;
 }
 
+// largest float t with (d2 <= t) <=> ((double)d2 <= D) for every float d2
+float float_floor(double D) {
+  float t = (float)D;
+  if ((double)t > D) t = nextafterf(t, -INFINITY);
+  return t;
+}
+
 // dynamic shared memory of a kernel that runs the staged correspondence search with `threads` threads per CTA
 static inline size_t nn_stage_bytes(const CorrArgs& ca, int threads) {
   return ca.nn_mode ? (size_t)(threads / 32) * ((size_t)ca.nn_cap * sizeof(f4) + 16) : 0;
@@ -1476,6 +1483,104 @@ int lb_gicp_compute_normals_radius(lb_gicp* h, int which, double radius, const f
     LB_CUDA(cudaStreamSynchronize(c.stream));
   }
   if (n_valid) *n_valid = m;
+  return LB_OK;
+}
+
+namespace {
+// flags (original order) -> ascending indices of the flagged points; the count lands in S.h_u32[6] after the stream sync
+int compact_flags(Ctx& c, Scratch& S, const uint32_t* d_flags, uint32_t* d_pos, uint32_t N, int32_t* d_idx) {
+  uint32_t* d_tot = S.d_u32 + 6;
+  LB_TRY(exclusive_scan_u32(c, S.scan, d_flags, d_pos, N, d_tot));
+  compact_indices_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(d_flags, d_pos, N, d_idx);
+  c.launches++;
+  LB_CUDA(cudaGetLastError());
+  LB_CUDA(cudaMemcpyAsync(S.h_u32 + 6, d_tot, sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+  return LB_OK;
+}
+}  // namespace
+
+// Row f5: pcl::StatisticalOutlierRemoval (PointCloudFilter.cc:126-133).
+int lb_gicp_statistical_outlier_removal(lb_gicp* h, int which, int mean_k, double std_mul, int negative, int32_t* kept_idx,
+                                        size_t* n_kept, float* mean_dist, double* stats3, int mem) {
+  if (!h || !kept_idx || !n_kept || (which != 0 && which != 1)) { set_error("lb_gicp_statistical_outlier_removal: bad argument"); return LB_ERR_INVALID_ARG; }
+  *n_kept = 0;
+  Cloud& cl = which == 0 ? *h->src : *h->tgt;
+  if (!cl.valid) { set_error("lb_gicp_statistical_outlier_removal: no %s cloud", which == 0 ? "source" : "target"); return which == 0 ? LB_ERR_EMPTY_SOURCE : LB_ERR_NO_TARGET; }
+  if (mean_k < 1) { set_error("lb_gicp_statistical_outlier_removal: mean_k must be >= 1"); return LB_ERR_INVALID_ARG; }
+  if (mean_k > 19) { set_error("lb_gicp_statistical_outlier_removal: mean_k must be <= 19 (20 neighbours with the point itself)"); return LB_ERR_UNSUPPORTED; }
+  if (cl.n < (size_t)mean_k + 1) { set_error("lb_gicp_statistical_outlier_removal: cloud has %zu points, fewer than mean_k + 1 = %d", cl.n, mean_k + 1); return LB_ERR_TOO_FEW_POINTS; }
+  Scratch& S = h->sc[which];
+  Ctx& c = S.c;
+  LB_CUDA(cudaSetDevice(c.device));
+  LB_TRY(finish_index(h, cl, which));
+  const uint32_t N = (uint32_t)cl.n;
+  float* d_dist = mean_dist;
+  double* d_stats = stats3;
+  int32_t* d_idx = kept_idx;
+  if (mem == LB_MEM_HOST || !mean_dist) { LB_TRY(h->io_d2.ensure(N)); d_dist = h->io_d2.p; }
+  if (mem == LB_MEM_HOST || !stats3) { LB_TRY(h->M.ensure(3)); d_stats = h->M.p; }    // M: not in use outside align()
+  if (mem == LB_MEM_HOST) { LB_TRY(h->io_idx.ensure(N)); d_idx = h->io_idx.p; }
+  LB_TRY(S.worklist.ensure(N)); LB_TRY(S.keys.ensure(N));
+  cl.keys_slot = -1;                               // the slot's key scratch is reused as the flag array
+  uint32_t* d_wl = S.d_u32 + 4;
+  LB_CUDA(cudaMemsetAsync(d_wl, 0, 2 * sizeof(uint32_t), c.stream));
+  MeanDistFin fin;
+  fin.out = d_dist;
+  GridView v = cl.view();
+  static const int ring_cap = [] { const char* e = getenv("LB_RING_CAP"); return e ? atoi(e) : 6; }();
+  knn_cov_quadreg_kernel<20, MeanDistFin><<<cdiv(4ll * N, KQ_THREADS), KQ_THREADS, 0, c.stream>>>(v, cl.raw.p, mean_k + 1, fin, 99,
+                                                                                          ring_cap, S.worklist.p, d_wl, nullptr);
+  knn_cov_tail_kernel<20, MeanDistFin><<<c.sm_count * 2, 128, 0, c.stream>>>(v, mean_k + 1, fin, S.worklist.p, d_wl);
+  sor_stats_kernel<<<1, 256, 0, c.stream>>>(d_dist, N, std_mul, d_stats);
+  sor_flags_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(d_dist, N, d_stats, negative, S.keys.p);
+  c.launches += 4;
+  LB_CUDA(cudaGetLastError());
+  LB_TRY(compact_flags(c, S, S.keys.p, S.worklist.p, N, d_idx));
+  if (mem == LB_MEM_HOST && mean_dist) LB_CUDA(cudaMemcpyAsync(mean_dist, d_dist, (size_t)N * sizeof(float), cudaMemcpyDeviceToHost, c.stream));
+  if (mem == LB_MEM_HOST && stats3) LB_CUDA(cudaMemcpyAsync(stats3, d_stats, 3 * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+  LB_CUDA(cudaStreamSynchronize(c.stream));
+  const size_t m = S.h_u32[6];
+  if (mem == LB_MEM_HOST && m) {
+    LB_CUDA(cudaMemcpyAsync(kept_idx, d_idx, m * sizeof(int32_t), cudaMemcpyDeviceToHost, c.stream));
+    LB_CUDA(cudaStreamSynchronize(c.stream));
+  }
+  *n_kept = m;
+  return LB_OK;
+}
+
+// Row f5: pcl::RadiusOutlierRemoval (PointCloudFilter.cc:135-143, PointCloudMerger.cc:112-117,139-144,169-174).
+int lb_gicp_radius_outlier_removal(lb_gicp* h, int which, double radius, int min_neighbors, int dense, int negative,
+                                   int32_t* kept_idx, size_t* n_kept, int mem) {
+  if (!h || !kept_idx || !n_kept || (which != 0 && which != 1)) { set_error("lb_gicp_radius_outlier_removal: bad argument"); return LB_ERR_INVALID_ARG; }
+  *n_kept = 0;
+  if (!(radius > 0.0)) { set_error("lb_gicp_radius_outlier_removal: radius must be > 0"); return LB_ERR_INVALID_ARG; }
+  if (min_neighbors < 0) { set_error("lb_gicp_radius_outlier_removal: min_neighbors must be >= 0"); return LB_ERR_INVALID_ARG; }
+  Cloud& cl = which == 0 ? *h->src : *h->tgt;
+  if (!cl.valid) { set_error("lb_gicp_radius_outlier_removal: no %s cloud", which == 0 ? "source" : "target"); return which == 0 ? LB_ERR_EMPTY_SOURCE : LB_ERR_NO_TARGET; }
+  Scratch& S = h->sc[which];
+  Ctx& c = S.c;
+  LB_CUDA(cudaSetDevice(c.device));
+  LB_TRY(finish_index(h, cl, which));
+  const uint32_t N = (uint32_t)cl.n;
+  int32_t* d_idx = kept_idx;
+  if (mem == LB_MEM_HOST) { LB_TRY(h->io_idx.ensure(N)); d_idx = h->io_idx.p; }
+  LB_TRY(S.worklist.ensure(N)); LB_TRY(S.keys.ensure(N));
+  cl.keys_slot = -1;                               // the slot's key scratch is reused as the flag array
+  // at most N points can pass the test: a larger count is never reached either way
+  const int need = (size_t)min_neighbors + 1 > (size_t)N + 1 ? (int)N + 1 : min_neighbors + 1;
+  const double r2 = radius * radius;
+  if (dense) radius_count_kernel<false><<<cdiv(N, 256), 256, 0, c.stream>>>(cl.view(), float_floor(r2), need, negative, S.keys.p);
+  else radius_count_kernel<true><<<cdiv(N, 256), 256, 0, c.stream>>>(cl.view(), (float)r2, need, negative, S.keys.p);
+  c.launches++;
+  LB_CUDA(cudaGetLastError());
+  LB_TRY(compact_flags(c, S, S.keys.p, S.worklist.p, N, d_idx));
+  LB_CUDA(cudaStreamSynchronize(c.stream));
+  const size_t m = S.h_u32[6];
+  if (mem == LB_MEM_HOST && m) {
+    LB_CUDA(cudaMemcpyAsync(kept_idx, d_idx, m * sizeof(int32_t), cudaMemcpyDeviceToHost, c.stream));
+    LB_CUDA(cudaStreamSynchronize(c.stream));
+  }
+  *n_kept = m;
   return LB_OK;
 }
 

@@ -297,10 +297,12 @@ knn_cov_quad_kernel(GridView g, int k, double eps, double* __restrict__ cov, int
   }
 }
 
-// What a k-NN kernel does with the k neighbours of a query, visited in ascending (d2, index) order:
+// What a k-NN kernel does with the k neighbours of a query, visited in ascending (d2, index) order (add() gets each
+// neighbour and its float32 squared distance to the query):
 // CovFin  -> GICP covariance (gicp.hpp:85-154): double moments -> Jacobi -> regularised, written in sorted order;
 // NormalFin -> PCL NormalEstimation (SURVEY 8f row f2, hd.h): nine float accumulators -> eigen33 -> flipped normal +
-//              curvature, written at the point's ORIGINAL index.
+//              curvature, written at the point's ORIGINAL index;
+// MeanDistFin -> PCL StatisticalOutlierRemoval's first pass (row f5), written at the ORIGINAL index.
 struct CovFin {
   double eps;
   double* cov;
@@ -310,7 +312,7 @@ struct CovFin {
     sum[0] = sum[1] = sum[2] = 0.0;
     m2[0] = m2[1] = m2[2] = m2[3] = m2[4] = m2[5] = 0.0;
   }
-  __device__ __forceinline__ void add(const f4& pt) {
+  __device__ __forceinline__ void add(const f4& pt, float) {
     sum[0] += pt.x; sum[1] += pt.y; sum[2] += pt.z;
     m2[0] += pt.x * pt.x; m2[1] += pt.y * pt.x; m2[2] += pt.y * pt.y;
     m2[3] += pt.z * pt.x; m2[4] += pt.z * pt.y; m2[5] += pt.z * pt.z;
@@ -338,7 +340,7 @@ struct CovFinIncr {
     sum[0] = sum[1] = sum[2] = 0.0;
     m2[0] = m2[1] = m2[2] = m2[3] = m2[4] = m2[5] = 0.0;
   }
-  __device__ __forceinline__ void add(const f4& pt) {
+  __device__ __forceinline__ void add(const f4& pt, float) {
     sum[0] += pt.x; sum[1] += pt.y; sum[2] += pt.z;
     m2[0] += pt.x * pt.x; m2[1] += pt.y * pt.x; m2[2] += pt.y * pt.y;
     m2[3] += pt.z * pt.x; m2[4] += pt.z * pt.y; m2[5] += pt.z * pt.z;
@@ -360,11 +362,29 @@ struct NormalFin {
   NormalAccum acc;
   __device__ __forceinline__ bool skip(const f4&) const { return false; }
   __device__ __forceinline__ void reset() { acc.reset(); }
-  __device__ __forceinline__ void add(const f4& pt) { acc.add(pt.x, pt.y, pt.z); }
+  __device__ __forceinline__ void add(const f4& pt, float) { acc.add(pt.x, pt.y, pt.z); }
   __device__ __forceinline__ void finish(uint32_t, const f4& q, int k, bool writer) {
     float o[4];
     pcl_normal_from_accum(acc, k, q.x, q.y, q.z, vp, o);
     if (writer) out[float_to_bits(q.w)] = f4{o[0], o[1], o[2], o[3]};
+  }
+};
+
+// statistical_outlier_removal.hpp (PCL 1.10): k = mean_k + 1 neighbours, the query itself first; dist_sum (double) +=
+// sqrtf(d2) over neighbours 1..mean_k in ascending order (entry 0 is the query, or a twin of it: d2 = 0 either way);
+// distance = (float)(dist_sum / mean_k).  sqrtf is correctly rounded here (-prec-sqrt=true) and in the oracle.
+struct MeanDistFin {
+  float* out;          // original order
+  double sum;
+  int cnt;
+  __device__ __forceinline__ bool skip(const f4&) const { return false; }
+  __device__ __forceinline__ void reset() { sum = 0.0; cnt = 0; }
+  __device__ __forceinline__ void add(const f4&, float d2) {
+    if (cnt > 0) sum = sum + (double)sqrtf(d2);
+    cnt++;
+  }
+  __device__ __forceinline__ void finish(uint32_t, const f4& q, int k, bool writer) {
+    if (writer) out[float_to_bits(q.w)] = (float)(sum / (double)(k - 1));
   }
 };
 
@@ -462,7 +482,7 @@ __device__ __forceinline__ void knn_quad_query(const GridView& g, const f4* __re
       if (bd == hd && bo == ho) p++;                       // original indices are unique: exactly one lane pops
       found++;
       kth = bits_to_float((int32_t)bd);
-      fin.add(raw[bo]);
+      fin.add(raw[bo], kth);
     }
     if (found == k && kth < ring_bound2(g, r, minfrac)) { done = true; break; }
   }
@@ -542,7 +562,7 @@ knn_cov_tail_kernel(GridView g, int k, Fin fin, const uint32_t* __restrict__ wor
         if (lane == src_lane) p++;
         found++;
         kth = __uint_as_float((unsigned)(best >> 32));
-        fin.add(g.pts[bs]);
+        fin.add(g.pts[bs], kth);
       }
       if (found == k && kth < ring_bound2(g, r, minfrac)) break;
     }
@@ -670,6 +690,104 @@ __global__ void __launch_bounds__(256)
 compact_indices_kernel(const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t n, int32_t* __restrict__ out_idx) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n && flags[i]) out_idx[pos[i]] = (int32_t)i;
+}
+
+// Row f5, StatisticalOutlierRemoval's statistics, as PCL computes them: two double sums over the mean distances IN INPUT
+// ORDER (sum += distance; sq_sum += distance * distance, a float product), then mean = sum / n, variance = (sq_sum -
+// sum * sum / n) / (n - 1), threshold = mean + std_mul * sqrt(variance).  A parallel tree would change the last bits, so
+// one CTA stages tiles of 256 distances in shared memory (coalesced) while lane 0 of warp 0 and lane 0 of warp 1 run
+// the two serial chains over the previous tile, as ap_normalize_seq_kernel does.  stats3 = {mean, stddev, threshold}.
+__global__ void __launch_bounds__(256)
+sor_stats_kernel(const float* __restrict__ dist, uint32_t n, double std_mul, double* __restrict__ stats3) {
+  __shared__ float tile[2][256];
+  __shared__ double sq_sum;
+  const int tid = threadIdx.x;
+  double acc = 0.0;
+  const uint32_t ntiles = (n + 255u) / 256u;
+  for (uint32_t t = 0; t <= ntiles; t++) {
+    if (t < ntiles) {
+      const uint32_t i = t * 256u + (uint32_t)tid;
+      tile[t & 1][tid] = i < n ? dist[i] : 0.f;
+    }
+    if (t > 0 && (tid == 0 || tid == 32)) {
+      const uint32_t base = (t - 1) * 256u;
+      const int cnt = (int)min(256u, n - base);
+      const float* src = tile[(t - 1) & 1];
+      if (tid == 0) {
+        for (int k = 0; k < cnt; k++) acc = acc + (double)src[k];
+      } else {
+        for (int k = 0; k < cnt; k++) { const float d = src[k]; acc = acc + (double)(d * d); }
+      }
+    }
+    __syncthreads();
+  }
+  if (tid == 32) sq_sum = acc;
+  __syncthreads();
+  if (tid == 0) {
+    const double nd = (double)n;
+    const double mean = acc / nd;
+    const double variance = (sq_sum - acc * acc / nd) / (nd - 1.0);
+    const double stddev = sqrt(variance);
+    stats3[0] = mean; stats3[1] = stddev; stats3[2] = mean + std_mul * stddev;
+  }
+}
+
+// PCL removes a point iff distance > threshold (with setNegative: distance <= threshold); the float distance is compared
+// in double.  A NaN threshold (n == 1) removes nothing.
+__global__ void __launch_bounds__(256)
+sor_flags_kernel(const float* __restrict__ dist, uint32_t n, const double* __restrict__ stats3, int negative,
+                 uint32_t* __restrict__ flags) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double thr = stats3[2], d = (double)dist[i];
+  const bool removed = negative ? (d <= thr) : (d > thr);
+  flags[i] = removed ? 0u : 1u;
+}
+
+// Row f5, RadiusOutlierRemoval: a point is an inlier iff at least `need` (= min_neighbors + 1, itself included) points
+// pass the distance test; STRICT: d2 < thr (FLANN's radius search, thr = float(r^2)), else d2 <= thr (the k-NN branch's
+// !(r^2 < (double)d2), thr = the largest float not above r^2).  One thread per query, in the cell-sorted order: the
+// threads of a warp query neighbouring points, so they walk the same cell runs (L1 hits) and mostly stop in the first
+// cell, as soon as the count reaches `need`; only the shells ring_bound2 says can reach the radius are scanned.
+template <bool STRICT>
+__global__ void __launch_bounds__(256)
+radius_count_kernel(GridView g, float thr, int need, int negative, uint32_t* __restrict__ flags) {
+  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= (uint32_t)g.n) return;
+  const f4 q = g.pts[s];
+  int cx, cy, cz; float minfrac;
+  query_cell(g, q.x, q.y, q.z, cx, cy, cz, minfrac);
+  int r0, r1;
+  ring_range(g, cx, cy, cz, r0, r1);
+  int cnt = 0;
+  for (int r = r0; r <= r1 && cnt < need; r++) {
+    const int z0 = imax_(cz - r, 0), z1 = imin_(cz + r, g.nz - 1);
+    const int y0 = imax_(cy - r, 0), y1 = imin_(cy + r, g.ny - 1);
+    for (int z = z0; z <= z1 && cnt < need; z++) {
+      const bool zface = iabs_(z - cz) == r;
+      for (int y = y0; y <= y1 && cnt < need; y++) {
+        const bool face = zface || iabs_(y - cy) == r;
+        const int base = (z * g.ny + y) * g.nx;
+        const int nseg = face ? 1 : 2;
+        for (int sgm = 0; sgm < nseg && cnt < need; sgm++) {
+          int xa, xb;
+          if (face) { xa = imax_(cx - r, 0); xb = imin_(cx + r, g.nx - 1); }
+          else { xa = xb = (sgm == 0) ? cx - r : cx + r; if (xa < 0 || xa >= g.nx) continue; }
+          if (xa > xb) continue;
+          const uint32_t a = g.cell_start[base + xa], e = g.cell_start[base + xb + 1];
+          for (uint32_t i = a; i < e && cnt < need; i++) {
+            const f4 p = g.pts[i];
+            const float d2 = dist2(q.x, q.y, q.z, p.x, p.y, p.z);
+            cnt += (STRICT ? d2 < thr : d2 <= thr) ? 1 : 0;
+          }
+        }
+      }
+    }
+    const float lb2 = ring_bound2(g, r, minfrac);      // nothing beyond the scanned block is closer than this
+    if (STRICT ? lb2 >= thr : lb2 > thr) break;
+  }
+  const bool inlier = cnt >= need;
+  flags[float_to_bits(q.w)] = (inlier != (negative != 0)) ? 1u : 0u;
 }
 
 // K3': covariance from a stored normal (the reference's default mode when normals are present)

@@ -111,12 +111,37 @@ class B200Gicp {
     }
     return true;
   }
+  // pcl::StatisticalOutlierRemoval (PointCloudFilter.cc:126-133) / pcl::RadiusOutlierRemoval (PointCloudFilter.cc:135-143,
+  // PointCloudMerger.cc:112-117) on `cloud`, in place: the kept points stay, in input order.  `dense` is the cloud's
+  // is_dense (PCL's branch of the radius filter).  Like computeNormals, the cloud becomes the handle's source.
+  bool statisticalOutlierRemoval(std::vector<PointF>& cloud, int mean_k = 10, double std_mul = 1.0, bool negative = false) {
+    return filterInPlace(cloud, [&](int32_t* kept, size_t* m) {
+      return lb_gicp_statistical_outlier_removal(h_, 0, mean_k, std_mul, negative ? 1 : 0, kept, m, nullptr, nullptr, LB_MEM_HOST);
+    });
+  }
+  bool radiusOutlierRemoval(std::vector<PointF>& cloud, double radius = 0.15, int min_neighbors = 3, bool dense = true,
+                            bool negative = false) {
+    return filterInPlace(cloud, [&](int32_t* kept, size_t* m) {
+      return lb_gicp_radius_outlier_removal(h_, 0, radius, min_neighbors, dense ? 1 : 0, negative ? 1 : 0, kept, m, LB_MEM_HOST);
+    });
+  }
   const lb_gicp_result& result() const { return r_; }
   lb_gicp* handle() { return h_; }
 
  private:
   void apply() {
     if (lb_gicp_set_params(h_, &p_) != LB_OK) throw std::invalid_argument(lb_last_error_string());
+  }
+  template <class Run>
+  bool filterInPlace(std::vector<PointF>& cloud, Run&& run) {
+    if (lb_gicp_set_source(h_, cloud.data(), cloud.size(), sizeof(PointF), 0, LB_NO_NORMALS, LB_MEM_HOST) != LB_OK) return false;
+    n_src_ = cloud.size();
+    std::vector<int32_t> kept(cloud.size());
+    size_t m = 0;
+    if (run(kept.data(), &m) != LB_OK) return false;
+    for (size_t j = 0; j < m; j++) cloud[j] = cloud[(size_t)kept[j]];    // kept[j] >= j: a forward pass is safe
+    cloud.resize(m);
+    return true;
   }
   lb_gicp* h_ = nullptr;
   lb_gicp_params p_{};

@@ -189,6 +189,18 @@ if __name__ == "__main__":
 
 
 # ------------------------------------------------------------------------------------------ C3 / C4 / C5 workloads
+# sensor -> base_link mounts of the three lidars point_cloud_merger concatenates (PointCloudMerger.cc:150-178)
+LIDAR_MOUNTS = (pose_matrix([0.3, 0.0, 0.4], [0.0, 0.0, 0.0]),
+                pose_matrix([-0.2, 0.25, 0.3], [0.0, 0.05, 2.1]),
+                pose_matrix([-0.2, -0.25, 0.3], [0.0, 0.05, -2.1]))
+
+
+def merged_scan(seed, beams=64, az=2048):
+    """One sweep of the three lidars in base_link, concatenated in merger order, finite points only: float32 (n, 3),
+    n ~ 3 * 0.99 * beams * az (~390 k at 64 x 2048) -- the full-resolution cloud the merger's radius filter sees."""
+    return world_points(make_scene(seed), LIDAR_MOUNTS, seed, beams, az)
+
+
 def perturbed_prior(T, seed, t=0.05, r_deg=0.4):
     """the odometry estimate handed to scan-to-submap registration as its guess: the true pose off by a few
     centimetres / tenths of a degree (PointCloudLocalization.cc:181-200 pre-transforms the query with it)"""
