@@ -49,6 +49,8 @@
  *   lb_voxel_set_leaf_size        impl_.setLeafSize()      custom_voxel_grid.cc:62-73, 97-101
  *   lb_voxel_set_filter_limits    impl_.setFilterFieldName/Limits/LimitsNegative  custom_voxel_grid.cc:103-134
  *   lb_voxel_filter               impl_.setInputCloud + setIndices + filter()     custom_voxel_grid.cc:76-87
+ *   lb_voxel_extract_features     the `filtering/extract_features` branch of PointCloudFilter::Filter
+ *                                 point_cloud_filter/src/PointCloudFilter.cc:144-173 (run from locus/src/Locus.cc:450)
  *   lb_ndt_*                      pclomp::NormalDistributionsTransform behind `registration_method: ndt`
  *                                 PointCloudOdometry.cc:182-195, PointCloudLocalization.cc:267-280 (section NDT below)
  *   lb_odometry_submit/next       the per-scan chain of the lidar callback: filtered scan -> odometry_.SetLidar()
@@ -345,6 +347,35 @@ int lb_voxel_set_input_passthrough(lb_voxel* h, const char* field_name, double l
 int lb_voxel_filter_merged(lb_voxel* h, const lb_voxel_input* inputs, int n_inputs, uint32_t point_step,
                            const lb_field* fields, int n_fields, uint8_t* out, size_t out_capacity_pts, size_t* n_out,
                            int32_t* out_voxel_idx, int mem_in, int mem_out);
+/* SURVEY 8f row f6 -- LOAM-style feature extraction of the point-cloud filter (PointCloudFilter.cc:144-173,
+ * arrangePCLInScanLines + extractFeatures :179-515): scan-ring arrangement, curvature, per-region sharp / less-sharp /
+ * flat picks, a VoxelGrid of each ring's less-flat points, then the fixed rotation of Filter().  Semantics:
+ * locus_b200/csrc/features.h.  Defaults (lb_features_default_params) are the reference's hard-coded values
+ * (PointCloudFilter.h:79-96): 16 rings over [-15, 15] deg, scan period 0.1, curvature region 5, 6 regions, at most 2
+ * sharp / 20 less-sharp / 4 flat points per region, curvature threshold 0.1, less-flat leaf 0.2. */
+typedef struct lb_features_params {
+  int n_rings;                    /* 1..128 */
+  float lower_deg, upper_deg;     /* finite, lower < upper */
+  float scan_period;
+  int curvature_region;           /* 1..32 */
+  int n_feature_regions;          /* 1..1024 */
+  int max_corner_sharp, max_corner_less_sharp, max_surface_flat;   /* >= 0 */
+  float curvature_threshold;
+  float less_flat_leaf;           /* > 0 */
+} lb_features_params;
+/* n_less_sharp includes the sharp points, which the output holds twice, as the reference's does */
+typedef struct lb_features_result {
+  size_t n_arranged, n_sharp, n_less_sharp, n_flat, n_less_flat, n_out;
+} lb_features_result;
+int lb_features_default_params(lb_features_params* p);
+/* pts: n points of `stride` bytes with FLOAT32 x, y, z at xyz_off (host or device: mem_in).  out4: n_out points of
+ * four floats x, y, z, intensity (host or device: mem_out; a device buffer 16-byte aligned), in the order sharp,
+ * less-sharp, flat, less-flat.  n == 0 -> LB_ERR_EMPTY_SOURCE (the reference reads point 0 unconditionally); invalid
+ * params -> LB_ERR_INVALID_ARG; out_capacity < n_out -> LB_ERR_CAPACITY with r->n_out the size needed and nothing
+ * written.  The handle's VoxelGrid settings are neither read nor changed. */
+int lb_voxel_extract_features(lb_voxel* h, const void* pts, size_t n, size_t stride, size_t xyz_off, int mem_in,
+                              const lb_features_params* p, float* out4, size_t out_capacity, lb_features_result* r,
+                              int mem_out);
 int lb_voxel_launch_count(lb_voxel* h, uint64_t* n);
 int lb_voxel_kernel_time(lb_voxel* h, float* ms_total_last_call);
 /* CUDA-event duration per call (first launch .. result available), averaged over the calls since the last reset */

@@ -78,6 +78,18 @@ class VoxelInput(C.Structure):
     _fields_ = [("data", C.c_void_p), ("n_pts", C.c_size_t), ("transform", C.c_void_p)]
 
 
+class FeaturesParams(C.Structure):
+    _fields_ = [("n_rings", C.c_int), ("lower_deg", C.c_float), ("upper_deg", C.c_float), ("scan_period", C.c_float),
+                ("curvature_region", C.c_int), ("n_feature_regions", C.c_int), ("max_corner_sharp", C.c_int),
+                ("max_corner_less_sharp", C.c_int), ("max_surface_flat", C.c_int), ("curvature_threshold", C.c_float),
+                ("less_flat_leaf", C.c_float)]
+
+
+class FeaturesResult(C.Structure):
+    _fields_ = [("n_arranged", C.c_size_t), ("n_sharp", C.c_size_t), ("n_less_sharp", C.c_size_t), ("n_flat", C.c_size_t),
+                ("n_less_flat", C.c_size_t), ("n_out", C.c_size_t)]
+
+
 class Field(C.Structure):
     _fields_ = [("name", C.c_char * 32), ("offset", C.c_uint32), ("datatype", C.c_uint8), ("count", C.c_uint32)]
 
@@ -96,6 +108,7 @@ SYMBOLS = [
     "lb_voxel_get_leaf_size", "lb_voxel_set_filter_limits", "lb_voxel_set_min_points_per_voxel",
     "lb_voxel_set_downsample_all_data", "lb_voxel_set_body_filter", "lb_voxel_filter", "lb_voxel_launch_count", "lb_voxel_kernel_time",
     "lb_voxel_kernel_time_avg", "lb_voxel_set_input_passthrough", "lb_voxel_filter_merged",
+    "lb_features_default_params", "lb_voxel_extract_features",
     "lb_submap_create", "lb_submap_destroy", "lb_submap_clear", "lb_submap_insert", "lb_submap_crop_box", "lb_submap_size",
     "lb_submap_generation", "lb_submap_points", "lb_submap_neighbors", "lb_submap_launch_count", "lb_gicp_set_target_submap",
     "lb_odometry_create", "lb_odometry_destroy", "lb_odometry_voxel", "lb_odometry_gicp", "lb_odometry_depth",
@@ -187,6 +200,10 @@ def lib():
         L.lb_voxel_set_input_passthrough.argtypes = [vp, C.c_char_p, C.c_double, C.c_double, i32]
         L.lb_voxel_filter_merged.argtypes = [vp, C.POINTER(VoxelInput), i32, C.c_uint32, C.POINTER(Field), i32, vp, sz,
                                              C.POINTER(sz), vp, i32, i32]
+    if hasattr(L, "lb_voxel_extract_features"):
+        L.lb_features_default_params.argtypes = [C.POINTER(FeaturesParams)]
+        L.lb_voxel_extract_features.argtypes = [vp, vp, sz, sz, sz, i32, C.POINTER(FeaturesParams), vp, sz,
+                                                C.POINTER(FeaturesResult), i32]
     L.lb_voxel_launch_count.argtypes = [vp, u64p]
     L.lb_voxel_kernel_time.argtypes = [vp, C.POINTER(C.c_float)]
     L.lb_voxel_kernel_time_avg.argtypes = [vp, C.POINTER(C.c_float), u64p, i32]
@@ -592,6 +609,54 @@ class VoxelGridB200:
                                      C.c_void_p(int(d_out)), capacity, C.byref(n_out),
                                      C.c_void_p(int(d_vidx)) if d_vidx else None, LB_MEM_DEVICE, LB_MEM_DEVICE))
         return n_out.value
+
+    @staticmethod
+    def featureParams(**params):
+        """lb_features_params: the reference's defaults (PointCloudFilter.h:79-96) with `params` overriding fields"""
+        p = FeaturesParams()
+        _check(lib().lb_features_default_params(C.byref(p)))
+        for k, v in params.items():
+            if k not in dict(FeaturesParams._fields_):
+                raise TypeError("unknown feature parameter %r" % k)
+            setattr(p, k, v)
+        return p
+
+    def extractFeatures(self, xyz_or_blob, stride=None, xyz_off=0, out=None, **params):
+        """The `filtering/extract_features` branch of PointCloudFilter::Filter (SURVEY 8f row f6).
+        xyz_or_blob: an (n, >=3) float32 array (numpy on the host, or a contiguous CUDA tensor on the device), or a uint8
+        host blob of `stride`-byte points with x, y, z at xyz_off.  out: None (a host array is returned) or a float32
+        CUDA tensor of shape (capacity, 4) that receives the points on the device.  Returns (out (m, 4) float32
+        x, y, z, intensity -- a view of `out` when given --, counts dict)."""
+        p = self.featureParams(**params)
+        if hasattr(xyz_or_blob, "data_ptr"):                    # CUDA tensor: device input
+            t = xyz_or_blob
+            assert t.is_cuda and t.dim() == 2 and t.shape[1] >= 3 and t.is_contiguous() and t.element_size() == 4
+            src, n, mem_in = C.c_void_p(t.data_ptr()), t.shape[0], LB_MEM_DEVICE
+            stride = t.shape[1] * 4
+        else:
+            a = np.ascontiguousarray(xyz_or_blob)
+            if a.dtype == np.uint8:
+                if stride is None:
+                    raise ValueError("a byte blob needs its stride")
+                a = a.reshape(-1)
+                n = a.size // stride
+            else:
+                a = np.ascontiguousarray(a, dtype=np.float32)
+                assert a.ndim == 2 and a.shape[1] >= 3
+                n, stride = a.shape[0], a.shape[1] * 4
+            src, mem_in = _ptr(a), LB_MEM_HOST
+        r = FeaturesResult()
+        if out is None:
+            host = np.zeros((max(2 * n, 1), 4), np.float32)
+            _check(lib().lb_voxel_extract_features(self._h, src, n, stride, xyz_off, mem_in, C.byref(p), _ptr(host),
+                                                   host.shape[0], C.byref(r), LB_MEM_HOST))
+            res = host[: r.n_out].copy()
+        else:
+            assert out.is_cuda and out.dim() == 2 and out.shape[1] == 4 and out.is_contiguous() and out.element_size() == 4
+            _check(lib().lb_voxel_extract_features(self._h, src, n, stride, xyz_off, mem_in, C.byref(p),
+                                                   C.c_void_p(out.data_ptr()), out.shape[0], C.byref(r), LB_MEM_DEVICE))
+            res = out[: r.n_out]
+        return res, {k: int(getattr(r, k)) for k, _ in FeaturesResult._fields_}
 
     def launchCount(self):
         n = C.c_uint64(0)

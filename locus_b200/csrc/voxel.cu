@@ -23,6 +23,13 @@
 namespace lb {
 const char* last_error();
 
+// feature extraction (features.cu) runs on the handle's stream with scratch of its own
+struct FeatWork;
+FeatWork* feat_work_new();
+void feat_work_free(FeatWork* w);
+int feat_extract(Ctx& c, FeatWork* w, const void* pts, size_t n, size_t stride, size_t xyz_off, int mem_in,
+                 const lb_features_params* q, float* out4, size_t out_capacity, lb_features_result* res, int mem_out);
+
 constexpr int VG_MAX_FIELDS = 16;
 
 struct VoxelFieldsDev {
@@ -504,6 +511,7 @@ struct lb_voxel {
   int bits_hint = 32;           // sort passes to enqueue: the key width of the previous call, rounded up to whole passes
   SortWork sort;
   ScanWork scan;
+  FeatWork* feat = nullptr;     // created by the first lb_voxel_extract_features
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   float t_last_ms = 0.f;
   double t_sum_ms = 0.0;        // since the last lb_voxel_kernel_time_avg(reset)
@@ -541,6 +549,7 @@ int lb_voxel_destroy(lb_voxel* h) {
   h->seg_start.release(); h->keep.release(); h->slot.release(); h->rec.release();
   h->sort.ka.release(); h->sort.kb.release(); h->sort.va.release(); h->sort.vb.release(); h->sort.hist.release();
   h->sort.scan.sums.release(); h->scan.sums.release();
+  feat_work_free(h->feat);
   if (h->d_st) cudaFree(h->d_st);
   if (h->h_st) cudaFreeHost(h->h_st);
   if (h->ev0) cudaEventDestroy(h->ev0);
@@ -589,6 +598,23 @@ int lb_voxel_kernel_time_avg(lb_voxel* h, float* ms_avg, uint64_t* calls, int re
   if (calls) *calls = h->t_calls;
   if (reset) { h->t_sum_ms = 0.0; h->t_calls = 0; }
   return LB_OK;
+}
+
+int lb_features_default_params(lb_features_params* p) {
+  if (!p) return LB_ERR_INVALID_ARG;
+  p->n_rings = 16; p->lower_deg = -15.f; p->upper_deg = 15.f; p->scan_period = 0.1f;
+  p->curvature_region = 5; p->n_feature_regions = 6;
+  p->max_corner_sharp = 2; p->max_corner_less_sharp = 20; p->max_surface_flat = 4;
+  p->curvature_threshold = 0.1f; p->less_flat_leaf = 0.2f;
+  return LB_OK;
+}
+
+int lb_voxel_extract_features(lb_voxel* h, const void* pts, size_t n, size_t stride, size_t xyz_off, int mem_in,
+                              const lb_features_params* p, float* out4, size_t out_capacity, lb_features_result* r,
+                              int mem_out) {
+  if (!h) { set_error("lb_voxel_extract_features: null handle"); return LB_ERR_INVALID_ARG; }
+  if (!h->feat) h->feat = feat_work_new();
+  return feat_extract(h->c, h->feat, pts, n, stride, xyz_off, mem_in, p, out4, out_capacity, r, mem_out);
 }
 
 int lb_voxel_set_input_passthrough(lb_voxel* h, const char* field_name, double limit_min, double limit_max, int negative) {

@@ -236,6 +236,30 @@ class B200VoxelGrid {
     return (long)n_out;
   }
 
+  // The `filtering/extract_features` branch of PointCloudFilter::Filter (PointCloudFilter.cc:144-173, SURVEY 8f row
+  // f6): sharp, less-sharp, flat and less-flat points, rotated.  `out` gets x, y, z and intensity with zero normals and
+  // curvature, like the reference's default-constructed PointF.  params: nullptr = the reference's defaults.
+  // Returns LB_OK or the C ABI's status (out is then empty).
+  int extractFeatures(const PointF* in, size_t n, std::vector<PointF>& out, const lb_features_params* params = nullptr,
+                      lb_features_result* result = nullptr) {
+    lb_features_params p;
+    if (params) p = *params; else lb_features_default_params(&p);
+    lb_features_result r{};
+    std::vector<float> buf(8 * n);               // the output never exceeds 2n points
+    const int s = lb_voxel_extract_features(h_, in, n, sizeof(PointF), offsetof(PointF, x), LB_MEM_HOST, &p, buf.data(),
+                                            2 * n, &r, LB_MEM_HOST);
+    if (result) *result = r;
+    out.clear();
+    if (s != LB_OK) return s;
+    out.resize(r.n_out);
+    for (size_t i = 0; i < r.n_out; i++) {
+      PointF q{};
+      q.x = buf[4 * i]; q.y = buf[4 * i + 1]; q.z = buf[4 * i + 2]; q.intensity = buf[4 * i + 3];
+      out[i] = q;
+    }
+    return LB_OK;
+  }
+
  private:
   void push() { lb_voxel_set_filter_limits(h_, field_.empty() ? nullptr : field_.c_str(), lo_, hi_, neg_); }
   lb_voxel* h_ = nullptr;

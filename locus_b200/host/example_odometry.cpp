@@ -62,6 +62,16 @@ int main() {
   std::printf("ndt: converged=%d t=(%.4f %.4f %.4f) after %d Newton steps\n", (int)ndt.hasConverged(), Tn[3], Tn[7], Tn[11], ndt.getFinalNumIteration());
   if (!(ndt.hasConverged() && std::fabs(Tn[3] + 0.05f) < 1e-2f && std::fabs(Tn[7] + 0.05f) < 1e-2f)) return 9;
 
+  // `filtering/extract_features` (row f6) on the cube: its rings are short, so few points come out, but the call runs
+  B200VoxelGrid features;
+  std::vector<PointF> feats;
+  lb_features_result fr{};
+  if (features.extractFeatures(reference.data(), reference.size(), feats, nullptr, &fr) != LB_OK) {
+    std::printf("features failed: %s\n", lb_last_error_string());
+    return 10;
+  }
+  std::printf("features: %zu arranged, %zu out\n", fr.n_arranged, fr.n_out);
+
   // the pipelined chain: the same two clouds as PointCloud2 blobs of PointF records
   B200Odometry odo(0, 2, reference.size(), sizeof(PointF));
   odo.setLeafSize(0.01f);                                     // finer than the 0.1 m lattice: every point survives

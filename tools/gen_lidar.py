@@ -72,8 +72,8 @@ def trajectory(seed, n, t_step=0.3, r_step_deg=2.0):
     return poses
 
 
-def _ray_dirs(beams, az):
-    el = np.deg2rad(np.linspace(-24.8, 2.0, beams))
+def _ray_dirs(beams, az, elev_deg=(-24.8, 2.0)):
+    el = np.deg2rad(np.linspace(elev_deg[0], elev_deg[1], beams))
     a = np.linspace(0, 2 * np.pi, az, endpoint=False)
     ce, se = np.cos(el)[:, None], np.sin(el)[:, None]
     d = np.stack([ce * np.cos(a)[None, :], ce * np.sin(a)[None, :], se * np.ones_like(a)[None, :]], axis=-1)
@@ -111,10 +111,11 @@ def _cast(scene, o, d):
     return t
 
 
-def scan(scene, pose, seed, beams=64, az=2048, noise=0.02, dropout=0.01):
-    """One scan in the SENSOR frame.  returns uint8 blob (n*32,), n = beams*az."""
+def scan(scene, pose, seed, beams=64, az=2048, noise=0.02, dropout=0.01, elev_deg=(-24.8, 2.0)):
+    """One scan in the SENSOR frame.  returns uint8 blob (n*32,), n = beams*az.  elev_deg: the beams' elevation span
+    (a VLP-16 sweep: beams=16, az=1800, elev_deg=(-15.0, 15.0))."""
     rng = np.random.default_rng(seed)
-    d_s = _ray_dirs(beams, az)
+    d_s = _ray_dirs(beams, az, elev_deg)
     R = pose[:3, :3]
     o = pose[:3, 3]
     d_w = d_s @ R.T
