@@ -200,12 +200,15 @@ int lb_gicp_promote_source_to_target(lb_gicp* h);
  *   lb_gicp_prepare_source   enqueue index + covariances of the current source now (align would do it lazily)
  *   lb_gicp_share_source     a new reference to the prepared source (release it with lb_cloud_release)
  *   lb_gicp_set_target_cloud adopt a shared cloud as target (no copy; this handle's stream waits for its preparation)
+ *   lb_gicp_set_source_cloud adopt a shared cloud as source, likewise (lb_locus: scan k's cloud is odometry source k,
+ *                            odometry target k+1 and localization source k)
  * A shared cloud is immutable: a handle that still holds it and gets new data switches to another object.  The
  * handles must sit on the same device and use the same covariance parameters. */
 typedef struct lb_cloud lb_cloud;
 int lb_gicp_prepare_source(lb_gicp* h);
 int lb_gicp_share_source(lb_gicp* h, lb_cloud** out);
 int lb_gicp_set_target_cloud(lb_gicp* h, lb_cloud* cloud);
+int lb_gicp_set_source_cloud(lb_gicp* h, lb_cloud* cloud);
 int lb_cloud_release(lb_cloud* cloud);
 
 /* guess: row-major 4x4 float, NULL = identity (the callers pass none). */
@@ -482,6 +485,78 @@ int lb_odometry_launch_count(lb_odometry* h, uint64_t* n);
  * out6 = { scans filtered, VoxelGrid stage busy s, its wait s (for a scan or a free ring slot),
  *          scans registered, registration workers busy s (summed over workers), their wait s (for a filtered scan) } */
 int lb_odometry_stage_times(lb_odometry* h, double* out6);
+
+/* ------------------------------------------------- the whole lidar callback as one pipeline
+ * Locus::LidarCallback from raw scan to integrated pose and updated map (locus/src/Locus.cc:450-543): VoxelGrid ->
+ * scan-to-scan odometry (PointCloudOdometry::UpdateEstimate) -> MotionUpdate -> scan-to-submap GICP
+ * (PointCloudLocalization::MeasurementUpdate) -> keyframe test -> InsertPoints -> Refresh.  The lb_odometry pipeline
+ * runs the first two stages; a third stage (one host thread, one lb_gicp handle bound to the caller's lb_submap) takes
+ * the scans strictly in order and localizes them.  Each filtered scan's index and covariances are built once and shared
+ * by odometry source k, odometry target k+1 and localization source k.  The rolling submap stands in for the external
+ * mapper's neighbours as the localization target (the semantics of lb_gicp_set_target_submap).  Pose semantics and
+ * what is unpinned: locus_b200/csrc/lo_pose.h and DESIGN.md.
+ *
+ * Threading and buffers as lb_odometry: submit / next from one thread; a submitted scan stays valid until its result
+ * is returned.  The submap belongs to the caller but must not be used by anybody else while scans are in flight. */
+typedef struct lb_locus lb_locus;
+
+typedef struct lb_locus_thresholds {
+  int enabled;               /* transform_thresholding */
+  double max_translation;    /* metres, |t| <= max_translation */
+  double max_rotation;       /* radians, |ToEulerZYX| <= max_rotation */
+} lb_locus_thresholds;
+
+typedef struct lb_locus_params {
+  lb_gicp_params odometry;               /* k_correspondences, gicp_epsilon and index_cell_size must equal the */
+  lb_gicp_params localization;           /* localization's: the shared clouds serve both registrations */
+  lb_locus_thresholds odometry_thresholds;       /* point_cloud_odometry icp/transform_thresholding, max_* */
+  lb_locus_thresholds localization_thresholds;   /* point_cloud_localization localization/transform_thresholding, max_* */
+  double translation_threshold_kf;       /* keyframe when |t| of PoseDelta(last keyframe, pose) exceeds it ... */
+  double rotation_threshold_kf;          /* ... or its 2 acos(q.w) does */
+  int add_keyframes;                     /* b_add_keyframes_enabled */
+  int refresh_every;                     /* >= 1: keyframes per Refresh (map_publishment/meters) */
+  int msw;                               /* b_enable_msw: Refresh crops the map to the window */
+  float window_half_size;                /* > 0: crop box centre = pose translation, +- this on every axis */
+  int prior_map;                         /* b_run_with_gt_point_cloud: localize the first scan against the caller's map */
+  double initial_pose[16];               /* row-major; L and the last keyframe before the first scan */
+} lb_locus_params;
+
+typedef struct lb_locus_result {
+  uint64_t ticket;
+  int status;                      /* lb_status of the scan's first failing stage */
+  char error[160];
+  size_t n_filtered;
+  int has_odometry;                /* 0 for the first scan and the scan after a failed one (no odometry target) */
+  lb_gicp_result odometry;
+  int odometry_accepted;           /* the increment passed the odometry thresholds (O moved) */
+  int has_localization;
+  lb_gicp_result localization;
+  int correction_accepted;         /* the localization correction passed its thresholds */
+  double odometry_pose[16];        /* O_k, row-major, after this scan */
+  double incremental[16];          /* I_k: what localization received (also when the odometry thresholds discarded it) */
+  double pose[16];                 /* L_k: the integrated localization estimate */
+  int keyframe;                    /* the scan was inserted into the map (the first scan or a keyframe) */
+  size_t n_inserted, n_removed;    /* map points added by the insert / removed by the crop of this scan */
+  size_t map_size;                 /* after this scan */
+} lb_locus_result;
+
+/* the reference's shipped values: locus/config/lo_settings.yaml, point_cloud_odometry/config/parameters.yaml,
+ * point_cloud_localization/config/parameters.yaml; odometry align_points_per_cta = 1024 (DESIGN.md, SM budget) */
+int lb_locus_default_params(lb_locus_params* p);
+/* depth: odometry workers (1..16); `map` on `device`, owned by the caller and outliving the handle */
+int lb_locus_create(int device, int depth, size_t max_points, uint32_t max_point_step, lb_submap* map, lb_locus** out);
+/* joins every stage; scans still in flight are dropped */
+int lb_locus_destroy(lb_locus* h);
+lb_voxel* lb_locus_voxel(lb_locus* h);
+/* refused while scans are in flight, and when the two gicp params disagree on the shared clouds */
+int lb_locus_set_params(lb_locus* h, const lb_locus_params* p);
+/* same arguments and blocking rule as lb_odometry_submit; guess = the odometry prior */
+int lb_locus_submit(lb_locus* h, const uint8_t* scan, size_t n_pts, uint32_t point_step, const lb_field* fields,
+                    int n_fields, int mem, const float* guess, uint8_t* filtered_out, int mem_filtered, uint64_t* ticket);
+int lb_locus_next(lb_locus* h, lb_locus_result* r, int block);
+int lb_locus_pending(lb_locus* h, size_t* n);
+/* out9 = the six values of lb_odometry_stage_times, then { scans localized, localization stage busy s, its wait s } */
+int lb_locus_stage_times(lb_locus* h, double* out9);
 
 /* ------------------------------------------------------------------ NDT (SURVEY 8f row f4)
  * LOCUS's alternative registration method (`registration_method: ndt`, registration_settings.h:3-12): the OpenMP NDT

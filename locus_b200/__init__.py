@@ -12,5 +12,5 @@ can be checked), but creating a handle without a CUDA device raises.
 from .api import (  # noqa: F401
     LocusB200Error, lib, lib_path, build, GicpB200, VoxelGridB200, SubmapB200, OdometryB200, OdometryResult, NdtB200, NdtParams, NdtResult, NDT_KDTREE, NDT_DIRECT26, NDT_DIRECT7, NDT_DIRECT1, GicpParams, GicpResult,
     LB_MEM_HOST, LB_MEM_DEVICE, LB_OPT_BFGS, LB_OPT_GAUSS_NEWTON, LB_EXEC_PERSISTENT, LB_EXEC_HOST_DRIVEN, LB_EXEC_PERSISTENT_CLUSTER, LB_EXEC_STREAM_ORDERED,
-    device_count, xyzi_fields,
+    device_count, xyzi_fields, LocusB200, LocusParams, LocusResult, locus_params,
 )

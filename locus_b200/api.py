@@ -74,6 +74,25 @@ class OdometryResult(C.Structure):
                 ("gicp", GicpResult), ("error", C.c_char * 160)]
 
 
+class LocusThresholds(C.Structure):
+    _fields_ = [("enabled", C.c_int), ("max_translation", C.c_double), ("max_rotation", C.c_double)]
+
+
+class LocusParams(C.Structure):
+    _fields_ = [("odometry", GicpParams), ("localization", GicpParams), ("odometry_thresholds", LocusThresholds),
+                ("localization_thresholds", LocusThresholds), ("translation_threshold_kf", C.c_double),
+                ("rotation_threshold_kf", C.c_double), ("add_keyframes", C.c_int), ("refresh_every", C.c_int),
+                ("msw", C.c_int), ("window_half_size", C.c_float), ("prior_map", C.c_int), ("initial_pose", C.c_double * 16)]
+
+
+class LocusResult(C.Structure):
+    _fields_ = [("ticket", C.c_uint64), ("status", C.c_int), ("error", C.c_char * 160), ("n_filtered", C.c_size_t),
+                ("has_odometry", C.c_int), ("odometry", GicpResult), ("odometry_accepted", C.c_int),
+                ("has_localization", C.c_int), ("localization", GicpResult), ("correction_accepted", C.c_int),
+                ("odometry_pose", C.c_double * 16), ("incremental", C.c_double * 16), ("pose", C.c_double * 16),
+                ("keyframe", C.c_int), ("n_inserted", C.c_size_t), ("n_removed", C.c_size_t), ("map_size", C.c_size_t)]
+
+
 class VoxelInput(C.Structure):
     _fields_ = [("data", C.c_void_p), ("n_pts", C.c_size_t), ("transform", C.c_void_p)]
 
@@ -100,6 +119,7 @@ SYMBOLS = [
     "lb_gicp_default_params", "lb_gicp_create", "lb_gicp_create_on_stream", "lb_gicp_destroy",
     "lb_gicp_set_params", "lb_gicp_get_params", "lb_gicp_set_source", "lb_gicp_set_target",
     "lb_gicp_promote_source_to_target", "lb_gicp_reserve", "lb_gicp_prepare_source", "lb_gicp_share_source", "lb_gicp_set_target_cloud",
+    "lb_gicp_set_source_cloud",
     "lb_cloud_release", "lb_gicp_align", "lb_gicp_transform_source", "lb_gicp_nn_target",
     "lb_gicp_fitness", "lb_gicp_point2plane_information", "lb_gicp_compute_normals", "lb_gicp_compute_normals_radius",
     "lb_gicp_statistical_outlier_removal", "lb_gicp_radius_outlier_removal", "lb_gicp_get_covariances", "lb_gicp_cloud_size", "lb_gicp_launch_count",
@@ -114,6 +134,8 @@ SYMBOLS = [
     "lb_odometry_create", "lb_odometry_destroy", "lb_odometry_voxel", "lb_odometry_gicp", "lb_odometry_depth",
     "lb_odometry_set_gicp_params", "lb_odometry_set_cloud_sharing", "lb_odometry_submit", "lb_odometry_next", "lb_odometry_pending",
     "lb_odometry_launch_count", "lb_odometry_stage_times",
+    "lb_locus_default_params", "lb_locus_create", "lb_locus_destroy", "lb_locus_voxel", "lb_locus_set_params", "lb_locus_submit",
+    "lb_locus_next", "lb_locus_pending", "lb_locus_stage_times",
     "lb_ndt_default_params", "lb_ndt_create", "lb_ndt_create_on_stream", "lb_ndt_destroy", "lb_ndt_set_params", "lb_ndt_set_source",
     "lb_ndt_set_target", "lb_ndt_align", "lb_ndt_target_voxels", "lb_ndt_derivatives", "lb_ndt_launch_count",
 ]
@@ -166,6 +188,8 @@ def lib():
         L.lb_gicp_prepare_source.argtypes = [vp]
         L.lb_gicp_share_source.argtypes = [vp, C.POINTER(vp)]
         L.lb_gicp_set_target_cloud.argtypes = [vp, vp]
+        if hasattr(L, "lb_gicp_set_source_cloud"):
+            L.lb_gicp_set_source_cloud.argtypes = [vp, vp]
         L.lb_cloud_release.argtypes = [vp]
     L.lb_gicp_align.argtypes = [vp, vp, C.POINTER(GicpResult)]
     L.lb_gicp_transform_source.argtypes = [vp, vp, vp, sz, sz, C.c_ssize_t, i32]
@@ -233,6 +257,16 @@ def lib():
         L.lb_odometry_pending.argtypes = [vp, C.POINTER(sz)]
         L.lb_odometry_launch_count.argtypes = [vp, u64p]
         L.lb_odometry_stage_times.argtypes = [vp, C.POINTER(C.c_double)]
+    if hasattr(L, "lb_locus_create"):
+        L.lb_locus_default_params.argtypes = [C.POINTER(LocusParams)]
+        L.lb_locus_create.argtypes = [i32, i32, sz, C.c_uint32, vp, C.POINTER(vp)]
+        L.lb_locus_destroy.argtypes = [vp]
+        L.lb_locus_voxel.argtypes = [vp]; L.lb_locus_voxel.restype = vp
+        L.lb_locus_set_params.argtypes = [vp, C.POINTER(LocusParams)]
+        L.lb_locus_submit.argtypes = [vp, vp, sz, C.c_uint32, C.POINTER(Field), i32, i32, vp, vp, i32, u64p]
+        L.lb_locus_next.argtypes = [vp, C.POINTER(LocusResult), i32]
+        L.lb_locus_pending.argtypes = [vp, C.POINTER(sz)]
+        L.lb_locus_stage_times.argtypes = [vp, C.POINTER(C.c_double)]
     if hasattr(L, "lb_ndt_create"):
         L.lb_ndt_default_params.argtypes = [C.POINTER(NdtParams)]
         L.lb_ndt_default_params.restype = None
@@ -374,6 +408,10 @@ class GicpB200:
 
     def setTargetCloud(self, cloud):
         _check(lib().lb_gicp_set_target_cloud(self._h, cloud))
+
+    def setSourceCloud(self, cloud):
+        """adopt a shared prepared cloud as source (no copy; the handle keeps its own reference)"""
+        _check(lib().lb_gicp_set_source_cloud(self._h, cloud))
 
     @staticmethod
     def releaseCloud(cloud):
@@ -832,6 +870,98 @@ class OdometryB200:
         _check(lib().lb_odometry_stage_times(self._h, a))
         return {"filtered": int(a[0]), "voxel_busy_s": a[1], "voxel_wait_s": a[2], "registered": int(a[3]),
                 "workers_busy_s": a[4], "workers_wait_s": a[5]}
+
+
+def locus_params(**kw):
+    """lb_locus_params with the reference's shipped values; keywords override top-level fields, and `odometry` /
+    `localization` / `*_thresholds` take dicts of their fields"""
+    p = LocusParams()
+    _check(lib().lb_locus_default_params(C.byref(p)))
+    for k, v in kw.items():
+        if k not in dict(LocusParams._fields_):
+            raise AttributeError(k)
+        if isinstance(v, dict):
+            sub = getattr(p, k)
+            for kk, vv in v.items():
+                if not hasattr(sub, kk):
+                    raise AttributeError("%s.%s" % (k, kk))
+                setattr(sub, kk, vv)
+        elif k == "initial_pose":
+            p.initial_pose[:] = [float(x) for x in np.asarray(v, dtype=np.float64).reshape(16)]
+        else:
+            setattr(p, k, v)
+    return p
+
+
+class LocusB200:
+    """Locus::LidarCallback (locus/src/Locus.cc:450-543) as one pipeline: VoxelGrid, scan-to-scan odometry,
+    scan-to-submap localization and keyframe map updates of `submap` (a SubmapB200 on the same device, which the
+    chain updates and the caller keeps).  Results come back in submission order with O_k, I_k and L_k as 4x4 doubles."""
+
+    def __init__(self, submap, device=0, depth=3, max_points=1 << 18, max_point_step=32, **params):
+        self._h = C.c_void_p()
+        _check(lib().lb_locus_create(device, depth, max_points, max_point_step, submap._h, C.byref(self._h)))
+        self.submap = submap
+        self.voxel = VoxelGridB200.__new__(VoxelGridB200)          # borrowed handle: never destroyed from here
+        self.voxel._h = C.c_void_p(lib().lb_locus_voxel(self._h)); self.voxel._borrowed = True
+        self._keep = {}
+        if params:
+            self.setParams(**params)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            lib().lb_locus_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def setParams(self, **kw):
+        """keywords as locus_params(); only while no scan is in flight"""
+        p = locus_params(**kw)
+        _check(lib().lb_locus_set_params(self._h, C.byref(p)))
+        self.params = p
+
+    def submit(self, scan, n_pts, point_step, fields, mem=LB_MEM_HOST, guess=None, filtered_out=None,
+               mem_filtered=LB_MEM_HOST):
+        """as OdometryB200.submit; guess = the odometry prior.  Returns the ticket."""
+        fa = fields if not isinstance(fields, (list, tuple)) else VoxelGridB200._fields(fields)
+        t = C.c_uint64(0)
+        g = None if guess is None else np.ascontiguousarray(guess, dtype=np.float32).reshape(16)
+        _check(lib().lb_locus_submit(self._h, _ptr(scan), n_pts, point_step, fa, len(fa), mem, _ptr(g),
+                                     _ptr(filtered_out), mem_filtered, C.byref(t)))
+        self._keep[t.value] = (scan, fa, g, filtered_out)
+        return t.value
+
+    def next(self, block=True):
+        """next LocusResult in submission order, or None when block=False and it is not ready."""
+        r = LocusResult()
+        s = lib().lb_locus_next(self._h, C.byref(r), int(bool(block)))
+        if s == 1:
+            return None
+        _check(s)
+        self._keep.pop(r.ticket, None)
+        return r
+
+    def pending(self):
+        n = C.c_size_t(0)
+        _check(lib().lb_locus_pending(self._h, C.byref(n)))
+        return n.value
+
+    def stageTimes(self):
+        a = (C.c_double * 9)()
+        _check(lib().lb_locus_stage_times(self._h, a))
+        return {"filtered": int(a[0]), "voxel_busy_s": a[1], "voxel_wait_s": a[2], "registered": int(a[3]),
+                "workers_busy_s": a[4], "workers_wait_s": a[5], "localized": int(a[6]), "localization_busy_s": a[7],
+                "localization_wait_s": a[8]}
+
+    @staticmethod
+    def poses(r):
+        """(O_k, I_k, L_k) of a LocusResult as 4x4 float64 arrays"""
+        return tuple(np.array(getattr(r, k), dtype=np.float64).reshape(4, 4) for k in ("odometry_pose", "incremental", "pose"))
 
 
 NDT_KDTREE, NDT_DIRECT26, NDT_DIRECT7, NDT_DIRECT1 = 0, 1, 2, 3

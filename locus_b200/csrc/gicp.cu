@@ -968,6 +968,19 @@ int lb_gicp_set_target_cloud(lb_gicp* h, lb_cloud* c) {
   return LB_OK;
 }
 
+// The source counterpart.  Nothing on the align, transform_source, nn_target or fitness paths writes into the source
+// object once it is prepared: prepare_clouds only builds what index_dirty / cov_valid say is missing, and the align
+// kernels transform a copy (src_work).  The next set_source / promote switches this handle to a private object first.
+int lb_gicp_set_source_cloud(lb_gicp* h, lb_cloud* c) {
+  if (!h || !c || !c->c) { set_error("lb_gicp_set_source_cloud: null argument"); return LB_ERR_INVALID_ARG; }
+  if (c->c->device != h->c.device) { set_error("lb_gicp_set_source_cloud: cloud lives on device %d, handle on %d", c->c->device, h->c.device); return LB_ERR_INVALID_ARG; }
+  LB_CUDA(cudaSetDevice(h->c.device));
+  if (h->src.use_count() > 1 && h->src != c->c) pool_release(h, h->src);   // my give-away stays recyclable
+  h->src = c->c;
+  LB_CUDA(cudaStreamWaitEvent(h->c.stream, h->src->ready, 0));
+  return LB_OK;
+}
+
 int lb_gicp_align(lb_gicp* h, const float* guess_in, lb_gicp_result* out) {
   if (!h || !out) { set_error("lb_gicp_align: null argument"); return LB_ERR_INVALID_ARG; }
   memset(out, 0, sizeof(*out));

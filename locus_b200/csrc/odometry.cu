@@ -12,6 +12,10 @@
 // exists because one align() is a chain of latency-bound kernels on a fraction of the SMs: the rest of the GPU filters
 // and indexes the following scans, and several aligns (each on its own CTAs) are in flight at once.  Results are
 // those of the sequential calls: registration k reads only filtered clouds k and k-1 and its caller-given prior.
+//
+// lb_locus_* (end of this file) runs the same core with a third stage L behind stage G: one thread, one lb_gicp handle
+// bound to the caller's lb_submap, localizing the scans strictly in order (pose semantics: lo_pose.h).  In that mode a
+// ticket is done when stage L has finished it, so stages V and G run at most the usual in-flight bound ahead of it.
 #include <chrono>
 #include <condition_variable>
 #include <cstdio>
@@ -22,11 +26,14 @@
 #include <thread>
 #include <vector>
 
-#ifdef LB_ODOMETRY_STUB          // TEST-ONLY build without CUDA: tests/odometry_harness.cpp supplies fake stages
+#if defined(LB_LOCUS_STUB)       // TEST-ONLY build without CUDA: tests/locus_harness.cpp supplies fake stages
+#include "locus_stub.h"
+#elif defined(LB_ODOMETRY_STUB)  // TEST-ONLY build without CUDA: tests/odometry_harness.cpp supplies fake stages
 #include "odometry_stub.h"
 #else
 #include "prims.cuh"
 #endif
+#include "lo_pose.h"
 
 using namespace lb;
 
@@ -65,7 +72,10 @@ struct Entry {           // per in-flight ticket
   Job job;
   lb_odometry_result res;
   bool filtered = false; // stage V done
-  bool done = false;     // stage G done (result complete)
+  bool aligned = false;  // stage G done (lb_locus only)
+  bool done = false;     // result complete: stage G done, or stage L with lb_locus
+  lb_cloud* loc_cloud = nullptr;   // lb_locus: stage L's reference to this scan's prepared cloud
+  lb_locus_result loc;             // lb_locus: filled by stage L
 };
 
 }  // namespace
@@ -80,6 +90,7 @@ struct lb_odometry {
   std::vector<Slot> ring;
   std::vector<Prepared> prep;          // same indexing as ring (ticket % R); used when share is on
   bool share = true;                   // lb_odometry_set_cloud_sharing (on by default)
+  bool chain = false;                  // run by lb_locus: stage L completes the tickets
   cudaStream_t copy_stream = nullptr;
   cudaStream_t voxel_stream = nullptr;
 
@@ -194,6 +205,9 @@ void align_stage(lb_odometry* h, int w) {
         st = lb_gicp_set_source(g, cur.d, cur.n, cur.point_step, (size_t)cur.xyz_off, LB_NO_NORMALS, LB_MEM_DEVICE);
         if (st == LB_OK) st = lb_gicp_prepare_source(g);
         if (st == LB_OK) st = lb_gicp_share_source(g, &mine);
+        // the chain's stage L adopts the same cloud as its localization source: its reference, not the ring slot,
+        // keeps the points alive until stage L is done with them
+        if (st == LB_OK && h->chain) st = lb_gicp_share_source(g, &e->loc_cloud);
         if (st != LB_OK) { r.status = st; copy_err(r.error, sizeof(r.error)); }
       }
       lb_cloud* prev = nullptr;
@@ -236,8 +250,12 @@ void align_stage(lb_odometry* h, int w) {
     }
     {
       std::lock_guard<std::mutex> lk(h->mu);
-      e->done = true;
-      advance_done_floor(h);
+      if (h->chain) {
+        e->aligned = true;
+      } else {
+        e->done = true;
+        advance_done_floor(h);
+      }
       h->t_worker_wait += std::chrono::duration<double>(tb0 - tw0).count();
       h->t_worker_busy += std::chrono::duration<double>(std::chrono::steady_clock::now() - tb0).count();
       h->n_registered++;
@@ -246,17 +264,13 @@ void align_stage(lb_odometry* h, int w) {
   }
 }
 
-}  // namespace
-
-extern "C" {
-
-int lb_odometry_create(int device, int depth, size_t max_points, uint32_t max_point_step, lb_odometry** out) {
+int odometry_create(int device, int depth, size_t max_points, uint32_t max_point_step, bool chain, lb_odometry** out) {
   if (!out || depth < 1 || depth > 16 || max_points == 0 || max_point_step < 12) {
     set_error("lb_odometry_create: need depth in 1..16, max_points > 0, max_point_step >= 12");
     return LB_ERR_INVALID_ARG;
   }
   lb_odometry* h = new lb_odometry;
-  h->device = device; h->depth = depth; h->max_points = max_points; h->max_step = max_point_step;
+  h->device = device; h->depth = depth; h->max_points = max_points; h->max_step = max_point_step; h->chain = chain;
   // The VoxelGrid stage is the one serial stage of the pipeline and a chain of ~12 short dependent kernels: on its
   // own high-priority stream its CTAs are placed before the pending CTAs of the workers' k-NN / index kernels.
   int st = LB_OK;
@@ -307,6 +321,34 @@ int lb_odometry_create(int device, int depth, size_t max_points, uint32_t max_po
   return LB_OK;
 }
 
+// the next ticket in submission order once it is done (mu not held); 1 = not done yet and block == 0
+int take_next(lb_odometry* h, int block, const char* who, Entry** out) {
+  Entry* e = nullptr;
+  {
+    std::unique_lock<std::mutex> lk(h->mu);
+    if (h->next_return == h->next_ticket) { set_error("%s: nothing pending", who); return LB_ERR_NO_ALIGN; }
+    e = h->inflight.front();
+    if (!e->done) {
+      if (!block) return 1;
+      h->cv.wait(lk, [&] { return e->done; });
+    }
+    h->inflight.pop_front();
+    h->next_return++;
+    advance_done_floor(h);
+  }
+  h->cv.notify_all();
+  *out = e;
+  return LB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int lb_odometry_create(int device, int depth, size_t max_points, uint32_t max_point_step, lb_odometry** out) {
+  return odometry_create(device, depth, max_points, max_point_step, false, out);
+}
+
 int lb_odometry_destroy(lb_odometry* h) {
   if (!h) return LB_OK;
   {
@@ -323,7 +365,10 @@ int lb_odometry_destroy(lb_odometry* h) {
   for (auto& s : h->ring) if (s.d) cudaFree(s.d);
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
   if (h->voxel_stream) cudaStreamDestroy(h->voxel_stream);
-  for (auto e : h->inflight) delete e;
+  for (auto e : h->inflight) {
+    if (e->loc_cloud) lb_cloud_release(e->loc_cloud);
+    delete e;
+  }
   delete h;
   return LB_OK;
 }
@@ -390,19 +435,8 @@ int lb_odometry_submit(lb_odometry* h, const uint8_t* scan, size_t n_pts, uint32
 int lb_odometry_next(lb_odometry* h, lb_odometry_result* r, int block) {
   if (!h || !r) { set_error("lb_odometry_next: null argument"); return LB_ERR_INVALID_ARG; }
   Entry* e = nullptr;
-  {
-    std::unique_lock<std::mutex> lk(h->mu);
-    if (h->next_return == h->next_ticket) { set_error("lb_odometry_next: nothing pending"); return LB_ERR_NO_ALIGN; }
-    e = h->inflight.front();
-    if (!e->done) {
-      if (!block) return 1;
-      h->cv.wait(lk, [&] { return e->done; });
-    }
-    h->inflight.pop_front();
-    h->next_return++;
-    advance_done_floor(h);
-  }
-  h->cv.notify_all();
+  const int st = take_next(h, block, "lb_odometry_next", &e);
+  if (st != LB_OK) return st;
   *r = e->res;
   delete e;
   return LB_OK;
@@ -433,3 +467,288 @@ int lb_odometry_launch_count(lb_odometry* h, uint64_t* n) {
 }
 
 }  // extern "C"
+
+// ================================================================ lb_locus_*: the whole lidar callback
+// The core above with stage L behind stage G.  Per ticket, in order, stage L adopts the scan's prepared cloud as the
+// source of its own lb_gicp handle, aligns it against the caller's rolling submap and does the pose bookkeeping and map
+// updates of Locus.cc:462-543 (lo_pose.h).  It is the one stage that depends on the previous scan's result, so it is the
+// only serial one; V and G fill and register the following scans meanwhile.
+#if !defined(LB_ODOMETRY_STUB) || defined(LB_LOCUS_STUB)
+
+namespace lb {
+int submap_device(const lb_submap* m);
+}
+
+struct lb_locus {
+  lb_odometry* core = nullptr;
+  lb_gicp* g = nullptr;            // stage L's handle (own stream); source = the shared cloud, target = the submap
+  lb_submap* map = nullptr;        // the caller's
+  float* d_xyz = nullptr;          // a keyframe's points in the fixed frame, max_points x 3 floats
+  lb_locus_params P;
+  // pose state, touched by stage L only (and by set_params while nothing is in flight)
+  bool started = false;            // the first scan has been taken
+  lo::Pose O, L, KF;               // odometry estimate, localization estimate, last keyframe
+  int counter = 0;                 // keyframes since the last Refresh
+  double t_busy = 0, t_wait = 0;   // core->mu held when updated
+  uint64_t n_localized = 0;
+  std::thread lthread;
+};
+
+namespace {
+
+int locus_insert(lb_locus* c, size_t n, lb_locus_result& r) {
+  float T[16];
+  lo::to_mat(c->L, T);
+  LB_TRY(lb_gicp_transform_source(c->g, T, c->d_xyz, 12, 0, LB_NO_NORMALS, LB_MEM_DEVICE));
+  size_t ins = 0;
+  LB_TRY(lb_submap_insert(c->map, c->d_xyz, n, 12, 0, LB_MEM_DEVICE, &ins, nullptr));
+  r.keyframe = 1;
+  r.n_inserted = ins;
+  return LB_OK;
+}
+
+// MotionUpdate(I) + MeasurementUpdate against the submap + the keyframe branch (PointCloudLocalization.cc:313-382,
+// Locus.cc:514-543)
+int locus_localize(lb_locus* c, const lo::Pose& I, size_t n, lb_locus_result& r) {
+  const lo::Pose P = lo::update(c->L, I);
+  float guess[16];
+  lo::to_mat(P, guess);
+  LB_TRY(lb_gicp_set_target_submap(c->g, c->map));
+  LB_TRY(lb_gicp_align(c->g, guess, &r.localization));
+  r.has_localization = 1;
+  const lo::Pose U = lo::delta(P, lo::from_mat(r.localization.final_transformation));   // sensor-frame correction
+  const lb_locus_thresholds& th = c->P.localization_thresholds;
+  r.correction_accepted = lo::passes(U, th.enabled, th.max_translation, th.max_rotation);
+  c->L = lo::update(c->L, r.correction_accepted ? lo::update(I, U) : I);
+  if (!c->P.add_keyframes || !lo::is_keyframe(lo::delta(c->KF, c->L), c->P.translation_threshold_kf, c->P.rotation_threshold_kf))
+    return LB_OK;
+  LB_TRY(locus_insert(c, n, r));
+  if (++c->counter == c->P.refresh_every) {
+    c->counter = 0;
+    if (c->P.msw) {
+      const float centre[3] = {(float)c->L.t[0], (float)c->L.t[1], (float)c->L.t[2]};
+      size_t removed = 0;
+      LB_TRY(lb_submap_crop_box(c->map, centre, c->P.window_half_size, &removed));
+      r.n_removed = removed;
+    }
+  }
+  c->KF = c->L;
+  return LB_OK;
+}
+
+void locus_scan(lb_locus* c, Entry* e) {
+  const lb_odometry_result& o = e->res;
+  lb_locus_result& r = e->loc;
+  memset(&r, 0, sizeof(r));
+  r.ticket = o.ticket; r.status = o.status; r.n_filtered = o.n_filtered;
+  memcpy(r.error, o.error, sizeof(r.error));
+  r.has_odometry = o.has_pose;
+  r.odometry = o.gicp;
+  lb_cloud* cl = e->loc_cloud;
+  e->loc_cloud = nullptr;
+  lo::Pose I = lo::identity();
+  // a failed voxel or odometry stage (or an empty filtered scan) changes no state
+  if (o.status == LB_OK && cl) {
+    int st = lb_gicp_set_source_cloud(c->g, cl);
+    if (st == LB_OK) {
+      if (o.has_pose) {
+        // PointCloudOdometry.cc:265-316: the increment is stored before the thresholds are tested, and localization
+        // receives it either way (Locus.cc:474)
+        I = lo::from_mat(o.gicp.final_transformation);
+        const lb_locus_thresholds& th = c->P.odometry_thresholds;
+        r.odometry_accepted = lo::passes(I, th.enabled, th.max_translation, th.max_rotation);
+        if (r.odometry_accepted) c->O = lo::update(c->O, I);
+      }
+      if (!c->started) {
+        // Locus.cc:462-472: the first scan seeds the map at the initial pose -- unless a prior map is loaded, in
+        // which case it is localized against it like any other scan (with I = identity)
+        c->started = true;
+        st = c->P.prior_map ? locus_localize(c, I, o.n_filtered, r) : locus_insert(c, o.n_filtered, r);
+      } else {
+        st = locus_localize(c, I, o.n_filtered, r);
+      }
+    }
+    if (st != LB_OK) { r.status = st; copy_err(r.error, sizeof(r.error)); }
+  }
+  if (cl) lb_cloud_release(cl);
+  lo::to_mat(c->O, r.odometry_pose);
+  lo::to_mat(I, r.incremental);
+  lo::to_mat(c->L, r.pose);
+  lb_submap_size(c->map, &r.map_size);
+}
+
+void loc_stage(lb_locus* c) {
+  lb_odometry* h = c->core;
+  cudaSetDevice(h->device);
+  for (uint64_t t = 0;; t++) {
+    Entry* e = nullptr;
+    const auto tw0 = std::chrono::steady_clock::now();
+    {
+      std::unique_lock<std::mutex> lk(h->mu);
+      h->cv.wait(lk, [&] { return h->stop || (t < h->next_ticket && h->entry(t)->aligned); });
+      if (h->stop) return;
+      e = h->entry(t);
+    }
+    const auto tb0 = std::chrono::steady_clock::now();
+    locus_scan(c, e);
+    {
+      std::lock_guard<std::mutex> lk(h->mu);
+      e->done = true;
+      advance_done_floor(h);
+      c->t_wait += std::chrono::duration<double>(tb0 - tw0).count();
+      c->t_busy += std::chrono::duration<double>(std::chrono::steady_clock::now() - tb0).count();
+      c->n_localized++;
+    }
+    h->cv.notify_all();
+  }
+}
+
+int locus_apply_params(lb_locus* c, const lb_locus_params* p) {
+  if (p->odometry.k_correspondences != p->localization.k_correspondences || p->odometry.gicp_epsilon != p->localization.gicp_epsilon ||
+      p->odometry.index_cell_size != p->localization.index_cell_size) {
+    set_error("lb_locus_set_params: odometry and localization must agree on k_correspondences, gicp_epsilon and "
+              "index_cell_size (each scan's index and covariances are built once for both)");
+    return LB_ERR_INVALID_ARG;
+  }
+  if (p->refresh_every < 1 || !(p->window_half_size > 0.f)) {
+    set_error("lb_locus_set_params: need refresh_every >= 1 and window_half_size > 0");
+    return LB_ERR_INVALID_ARG;
+  }
+  LB_TRY(lb_gicp_set_params(c->g, &p->localization));
+  int st = lb_odometry_set_gicp_params(c->core, &p->odometry);
+  if (st != LB_OK) {
+    lb_gicp_set_params(c->g, &c->P.localization);   // keep the previous state
+    return st;
+  }
+  c->P = *p;
+  if (!c->started) {
+    c->O = lo::identity();
+    c->L = c->KF = lo::from_mat(p->initial_pose);
+  }
+  return LB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int lb_locus_default_params(lb_locus_params* p) {
+  if (!p) { set_error("lb_locus_default_params: null argument"); return LB_ERR_INVALID_ARG; }
+  memset(p, 0, sizeof(*p));
+  // point_cloud_odometry/config/parameters.yaml icp/*, PointCloudOdometry.cc:147-155
+  lb_gicp_default_params(&p->odometry);
+  p->odometry.transformation_epsilon = 0.001;
+  p->odometry.max_correspondence_distance = 1.0;
+  p->odometry.max_iterations = 20;
+  p->odometry.ransac_iterations = 0;
+  p->odometry.euclidean_fitness_epsilon = 0.005;
+  p->odometry.align_points_per_cta = 1024;      // the chain's SM budget (DESIGN.md)
+  p->odometry_thresholds = {1, 1.0, 1.0};
+  // point_cloud_localization/config/parameters.yaml localization/*
+  lb_gicp_default_params(&p->localization);
+  p->localization.transformation_epsilon = 0.00001;
+  p->localization.max_correspondence_distance = 0.2;
+  p->localization.max_iterations = 20;
+  p->localization.ransac_iterations = 0;
+  p->localization_thresholds = {1, 1.0, 1.0};
+  // locus/config/lo_settings.yaml
+  p->translation_threshold_kf = 1.0;
+  p->rotation_threshold_kf = 0.3;
+  p->add_keyframes = 1;
+  p->refresh_every = 1;          // map_publishment/meters
+  p->msw = 1;                    // b_enable_msw
+  p->window_half_size = 20.f;    // box_filter_size
+  p->prior_map = 0;              // b_run_with_gt_point_cloud
+  for (int i = 0; i < 16; i++) p->initial_pose[i] = (i % 5 == 0) ? 1.0 : 0.0;
+  return LB_OK;
+}
+
+int lb_locus_create(int device, int depth, size_t max_points, uint32_t max_point_step, lb_submap* map, lb_locus** out) {
+  if (!out || !map) { set_error("lb_locus_create: null argument"); return LB_ERR_INVALID_ARG; }
+  if (lb::submap_device(map) != device) {
+    set_error("lb_locus_create: submap on device %d, chain on %d", lb::submap_device(map), device);
+    return LB_ERR_INVALID_ARG;
+  }
+  lb_locus* c = new lb_locus;
+  c->map = map;
+  lb_locus_params P;
+  lb_locus_default_params(&P);
+  int st = odometry_create(device, depth, max_points, max_point_step, true, &c->core);
+  if (st == LB_OK) st = lb_gicp_create(device, &c->g);
+  if (st == LB_OK) st = lb_gicp_reserve(c->g, max_points, 0);
+  if (st == LB_OK && cudaMalloc((void**)&c->d_xyz, max_points * 3 * sizeof(float)) != cudaSuccess) {
+    set_error("lb_locus_create: allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
+    st = LB_ERR_CUDA;
+  }
+  if (st == LB_OK) st = locus_apply_params(c, &P);
+  if (st != LB_OK) {
+    if (c->g) lb_gicp_destroy(c->g);
+    if (c->core) lb_odometry_destroy(c->core);
+    if (c->d_xyz) cudaFree(c->d_xyz);
+    delete c;
+    return st;
+  }
+  c->lthread = std::thread(loc_stage, c);
+  *out = c;
+  return LB_OK;
+}
+
+int lb_locus_destroy(lb_locus* c) {
+  if (!c) return LB_OK;
+  {
+    std::lock_guard<std::mutex> lk(c->core->mu);
+    c->core->stop = true;
+  }
+  c->core->cv.notify_all();
+  if (c->lthread.joinable()) c->lthread.join();
+  cudaSetDevice(c->core->device);
+  lb_gicp_destroy(c->g);
+  lb_odometry_destroy(c->core);    // joins stages V and G, releases the clouds of the scans still in flight
+  cudaFree(c->d_xyz);
+  delete c;
+  return LB_OK;
+}
+
+lb_voxel* lb_locus_voxel(lb_locus* c) { return c ? c->core->vg : nullptr; }
+
+int lb_locus_set_params(lb_locus* c, const lb_locus_params* p) {
+  if (!c || !p) { set_error("lb_locus_set_params: null argument"); return LB_ERR_INVALID_ARG; }
+  {
+    std::lock_guard<std::mutex> lk(c->core->mu);
+    if (c->core->next_return != c->core->next_ticket) { set_error("lb_locus_set_params: scans in flight"); return LB_ERR_INVALID_ARG; }
+  }
+  return locus_apply_params(c, p);
+}
+
+int lb_locus_submit(lb_locus* c, const uint8_t* scan, size_t n_pts, uint32_t point_step, const lb_field* fields,
+                    int n_fields, int mem, const float* guess, uint8_t* filtered_out, int mem_filtered, uint64_t* ticket) {
+  if (!c) { set_error("lb_locus_submit: null handle"); return LB_ERR_INVALID_ARG; }
+  return lb_odometry_submit(c->core, scan, n_pts, point_step, fields, n_fields, mem, guess, filtered_out, mem_filtered, ticket);
+}
+
+int lb_locus_next(lb_locus* c, lb_locus_result* r, int block) {
+  if (!c || !r) { set_error("lb_locus_next: null argument"); return LB_ERR_INVALID_ARG; }
+  Entry* e = nullptr;
+  const int st = take_next(c->core, block, "lb_locus_next", &e);
+  if (st != LB_OK) return st;
+  *r = e->loc;
+  delete e;
+  return LB_OK;
+}
+
+int lb_locus_pending(lb_locus* c, size_t* n) {
+  if (!c) return LB_ERR_INVALID_ARG;
+  return lb_odometry_pending(c->core, n);
+}
+
+int lb_locus_stage_times(lb_locus* c, double* out9) {
+  if (!c || !out9) return LB_ERR_INVALID_ARG;
+  LB_TRY(lb_odometry_stage_times(c->core, out9));
+  std::lock_guard<std::mutex> lk(c->core->mu);
+  out9[6] = (double)c->n_localized; out9[7] = c->t_busy; out9[8] = c->t_wait;
+  return LB_OK;
+}
+
+}  // extern "C"
+
+#endif  // lb_locus

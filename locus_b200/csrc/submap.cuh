@@ -39,6 +39,10 @@ struct lb_submap {
   uint64_t indexed_generation = ~0ull; // generation the engine's cloud was built from
 };
 
+namespace lb {
+int submap_device(const lb_submap* m) { return m->eng->c.device; }   // lb_locus_create checks it against its own
+}  // namespace lb
+
 namespace {
 
 template <class T>

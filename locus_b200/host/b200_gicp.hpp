@@ -304,4 +304,38 @@ class B200Odometry {
   lb_gicp_params p_{};
 };
 
+// The whole lidar callback (locus/src/Locus.cc:450-543) as the library's pipeline: VoxelGrid, odometry, localization
+// against `map` (the caller's lb_submap, updated with keyframes and cropped to the window), pose bookkeeping.
+class B200Locus {
+ public:
+  B200Locus(int device, int depth, size_t max_points, uint32_t max_point_step, lb_submap* map) {
+    if (lb_locus_create(device, depth, max_points, max_point_step, map, &h_) != LB_OK) throw std::runtime_error(lb_last_error_string());
+    lb_locus_default_params(&p_);
+  }
+  ~B200Locus() { lb_locus_destroy(h_); }
+  B200Locus(const B200Locus&) = delete;
+  B200Locus& operator=(const B200Locus&) = delete;
+
+  void setLeafSize(float l) { lb_voxel_set_leaf_size(lb_locus_voxel(h_), l, l, l); }
+  void setFilterLimits(const std::string& field, double lo, double hi) {
+    lb_voxel_set_filter_limits(lb_locus_voxel(h_), field.c_str(), lo, hi, 0);
+  }
+  lb_locus_params& params() { return p_; }                      // edit, then applyParams() while nothing is in flight
+  bool applyParams() { return lb_locus_set_params(h_, &p_) == LB_OK; }
+
+  // scan (and filtered_out, if given) must stay valid until next() has returned this ticket
+  bool submit(const uint8_t* scan, size_t n_pts, uint32_t point_step, const std::vector<lb_field>& fields,
+              const Matrix4f* prior = nullptr, uint8_t* filtered_out = nullptr, uint64_t* ticket = nullptr) {
+    return lb_locus_submit(h_, scan, n_pts, point_step, fields.data(), (int)fields.size(), LB_MEM_HOST,
+                           prior ? prior->data() : nullptr, filtered_out, LB_MEM_HOST, ticket) == LB_OK;
+  }
+  bool next(lb_locus_result* r, bool block = true) { return lb_locus_next(h_, r, block ? 1 : 0) == LB_OK; }
+  size_t pending() const { size_t n = 0; lb_locus_pending(h_, &n); return n; }
+  lb_locus* handle() { return h_; }
+
+ private:
+  lb_locus* h_ = nullptr;
+  lb_locus_params p_{};
+};
+
 }  // namespace locus_b200

@@ -91,5 +91,24 @@ int main() {
     return 6;
   }
   std::printf("pipeline: n_filtered=%zu t=(%.4f %.4f)\n", r1.n_filtered, r1.gicp.final_transformation[3], r1.gicp.final_transformation[7]);
-  return (std::fabs(r1.gicp.final_transformation[3] + 0.05f) < 1e-2f && std::fabs(r1.gicp.final_transformation[7] + 0.05f) < 1e-2f) ? 0 : 7;
+  if (!(std::fabs(r1.gicp.final_transformation[3] + 0.05f) < 1e-2f && std::fabs(r1.gicp.final_transformation[7] + 0.05f) < 1e-2f)) return 7;
+
+  // the whole callback: the first scan seeds the map, the second is odometry-aligned and localized against it
+  lb_submap* map = nullptr;
+  if (lb_submap_create(0, 0.05f, &map) != LB_OK) return 11;
+  int rc = 0;
+  {
+    B200Locus loc(0, 2, reference.size(), sizeof(PointF), map);
+    loc.setLeafSize(0.01f);
+    loc.params().odometry = odo.params();
+    loc.params().localization.max_correspondence_distance = 1.0;
+    if (!loc.applyParams()) rc = 12;
+    loc.submit(reinterpret_cast<const uint8_t*>(reference.data()), reference.size(), sizeof(PointF), fields);
+    loc.submit(reinterpret_cast<const uint8_t*>(query.data()), query.size(), sizeof(PointF), fields);
+    lb_locus_result l0, l1;
+    if (rc == 0 && (!loc.next(&l0) || !loc.next(&l1) || !l0.keyframe || !l1.has_localization || l1.status != LB_OK)) rc = 13;
+    if (rc == 0) std::printf("locus: L t=(%.4f %.4f), map %zu points\n", l1.pose[3], l1.pose[7], l1.map_size);
+  }
+  lb_submap_destroy(map);
+  return rc;
 }
