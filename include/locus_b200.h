@@ -240,6 +240,14 @@ int lb_gicp_point2plane_information(lb_gicp* h, const void* query, size_t n, siz
  * origin, what fromROSMsg leaves in sensor_origin_).  out4: n x (normal_x, normal_y, normal_z, curvature) float32 in
  * the caller's point order, host or device.  3 <= k <= 20.  (Radius mode: lb_gicp_compute_normals_radius.) */
 int lb_gicp_compute_normals(lb_gicp* h, int which, int k, const float* viewpoint, float* out4, int mem);
+/* The same normals, written into the cloud itself instead of a caller buffer: the NormalComputation nodelet in front of
+ * the registration (locus/launch/locus.launch:177-181).  Afterwards the source (which = 0) or target (1) has normals,
+ * exactly as if it had been uploaded with those normals at normal_off, and its covariances are invalidated: with
+ * recompute_source/target_covariance = 0 the next prepare_source / align takes them from the normals (gicp.hpp:81-82).
+ * A prepared source shared from here carries the normals, and lb_gicp_transform_source returns them rotated.  Errors as
+ * lb_gicp_compute_normals (3 <= k <= 20, at least k points), and the cloud is left as it was.  A cloud shared with
+ * another handle is refused (LB_ERR_INVALID_ARG): it is immutable. */
+int lb_gicp_estimate_normals(lb_gicp* h, int which, int k, const float* viewpoint);
 /* The nodelet's radius mode (normal_computation.cc:73-77, norm_est_.setRadiusSearch(normal_search_radius)) together
  * with the NaN-normal removal that follows it (:53-57, pcl::removeNaNNormalsFromPointCloud).  Neighbourhood of a point =
  * every point with squared distance < float(radius^2) (FLANN's strict compare), itself included, taken in ascending
@@ -411,19 +419,29 @@ int lb_submap_clear(lb_submap* m);
  * the `incremental_points` output of InsertPoints.  Non-finite points are skipped. */
 int lb_submap_insert(lb_submap* m, const void* pts, size_t n, size_t stride, size_t xyz_off, int mem, size_t* n_inserted,
                      float* inserted_xyz);
+/* lb_submap_insert for points with normals (float32 x,y,z at normal_off, fixed frame): the winning point of a voxel
+ * keeps its normal, and crops keep points and normals paired (Locus.cc:530-532 inserts the keyframe with its normals).
+ * Points inserted by lb_submap_insert have none. */
+int lb_submap_insert_with_normals(lb_submap* m, const void* pts, size_t n, size_t stride, size_t xyz_off, size_t normal_off,
+                                  int mem, size_t* n_inserted, float* inserted_xyz);
 int lb_submap_crop_box(lb_submap* m, const float* center3, float half_size, size_t* n_removed /* nullable */);
 int lb_submap_size(lb_submap* m, size_t* n);
 /* changes whenever the point set changed (insert that added points, crop that removed points, clear) */
 int lb_submap_generation(lb_submap* m, uint64_t* generation);
 /* the map's points, insertion order, n x 3 float32 */
 int lb_submap_points(lb_submap* m, float* xyz_out, size_t capacity_points, int mem);
+/* the map's normals, insertion order, n x 3 float32; NaN for points inserted without a normal */
+int lb_submap_normals(lb_submap* m, float* xyz_out, size_t capacity_points, int mem);
 /* neighbors_xyz (nullable): n x 3 float32, the nearest map point of every query; idx / d2 (nullable): its map index and
  * float32 squared distance.  All buffers host or all device (`mem`). */
 int lb_submap_neighbors(lb_submap* m, const void* query, size_t n, size_t stride, size_t xyz_off, float* neighbors_xyz,
                         int32_t* idx, float* d2, int mem);
 int lb_submap_launch_count(lb_submap* m, uint64_t* n);
 /* the submap as target of `h` (same device; k_correspondences <= 20).  Call again after the map changed; while it is
- * unchanged the call only checks the generation.  Uses h's k_correspondences / gicp_epsilon for the covariances. */
+ * unchanged the call only checks the generation.  Uses h's k_correspondences / gicp_epsilon for the covariances.
+ * With h's recompute_target_covariance = 0 and a normal on every map point, the covariances come from the stored
+ * normals instead (as for an uploaded cloud with normals), rebuilt only when the map or gicp_epsilon changed; otherwise
+ * the k-NN covariance cache is used. */
 int lb_gicp_set_target_submap(lb_gicp* h, lb_submap* m);
 
 /* ------------------------------------------------- scan-to-scan odometry pipeline
@@ -467,6 +485,12 @@ int lb_odometry_set_gicp_params(lb_odometry* h, const lb_gicp_params* p);
  * the reference do (setInputTarget clears the target's covariances, gicp.h:196-200).  Call while the pipeline is idle,
  * before the first scan. */
 int lb_odometry_set_cloud_sharing(lb_odometry* h, int on);
+/* Normals stage (OFF by default; k = 0).  3 <= k <= 20: the worker that prepares scan k's cloud gives it its k-NN
+ * normals (lb_gicp_estimate_normals, viewpoint NULL = the origin) before its index and covariances are built, so odometry
+ * source k, odometry target k+1 and lb_locus's localization source k all carry them; without cloud sharing the target
+ * gets its normals the same way.  Covariances come from them where the gicp params say recompute_*_covariance = 0.
+ * Call while the pipeline is idle, before the first scan. */
+int lb_odometry_set_normals(lb_odometry* h, int k, const float* viewpoint);
 /* scan: n_pts points of point_step bytes described by fields (as lb_voxel_filter); xyz must be FLOAT32 fields.
  * guess: row-major 4x4 prior handed to align() (NULL = identity).  filtered_out (nullable): host (LB_MEM_HOST) or
  * device buffer of at least n_pts * point_step bytes that receives the filtered cloud.  Blocks while 2*depth+2 scans
@@ -506,9 +530,23 @@ typedef struct lb_locus_thresholds {
   double max_rotation;       /* radians, |ToEulerZYX| <= max_rotation */
 } lb_locus_thresholds;
 
+/* The front end LOCUS ships in front of its callback; all 0 = off (lb_locus_default_params).  Shipped values:
+ * normals_k = 20 (NormalComputation nodelet, locus.launch:177-181, NormalComputation.cfg:13,15), adaptive_voxelization
+ * = 1 and points_to_process = 3000 (lo_settings.yaml:84-85). */
+typedef struct lb_locus_front_end {
+  int normals_k;              /* 0 = off; 3..20: every filtered scan gets its k-NN normals (lb_odometry_set_normals),
+                                 keyframes enter the map with their normals rotated into the fixed frame */
+  float viewpoint[3];         /* the normals' viewpoint, sensor frame (the origin in LOCUS) */
+  int adaptive_voxelization;  /* b_adaptive_input_voxelization: retune the VoxelGrid leaf after every filtered scan,
+                                 Locus.cc:780-810; the new leaf applies to the next scan */
+  int points_to_process;      /* points_to_process_in_callback: the filtered point count the leaf aims at (> 0) */
+} lb_locus_front_end;
+
 typedef struct lb_locus_params {
   lb_gicp_params odometry;               /* k_correspondences, gicp_epsilon and index_cell_size must equal the */
-  lb_gicp_params localization;           /* localization's: the shared clouds serve both registrations */
+  lb_gicp_params localization;           /* localization's: the shared clouds serve both registrations; so must the
+                                            odometry's two recompute_*_covariance and the localization's
+                                            recompute_source_covariance (one prepared cloud is all three) */
   lb_locus_thresholds odometry_thresholds;       /* point_cloud_odometry icp/transform_thresholding, max_* */
   lb_locus_thresholds localization_thresholds;   /* point_cloud_localization localization/transform_thresholding, max_* */
   double translation_threshold_kf;       /* keyframe when |t| of PoseDelta(last keyframe, pose) exceeds it ... */
@@ -519,6 +557,7 @@ typedef struct lb_locus_params {
   float window_half_size;                /* > 0: crop box centre = pose translation, +- this on every axis */
   int prior_map;                         /* b_run_with_gt_point_cloud: localize the first scan against the caller's map */
   double initial_pose[16];               /* row-major; L and the last keyframe before the first scan */
+  lb_locus_front_end front_end;          /* normals and adaptive input voxelization (off by default) */
 } lb_locus_params;
 
 typedef struct lb_locus_result {
@@ -538,6 +577,7 @@ typedef struct lb_locus_result {
   int keyframe;                    /* the scan was inserted into the map (the first scan or a keyframe) */
   size_t n_inserted, n_removed;    /* map points added by the insert / removed by the crop of this scan */
   size_t map_size;                 /* after this scan */
+  float leaf_size;                 /* the VoxelGrid x leaf this scan was filtered with */
 } lb_locus_result;
 
 /* the reference's shipped values: locus/config/lo_settings.yaml, point_cloud_odometry/config/parameters.yaml,
@@ -548,7 +588,8 @@ int lb_locus_create(int device, int depth, size_t max_points, uint32_t max_point
 /* joins every stage; scans still in flight are dropped */
 int lb_locus_destroy(lb_locus* h);
 lb_voxel* lb_locus_voxel(lb_locus* h);
-/* refused while scans are in flight, and when the two gicp params disagree on the shared clouds */
+/* refused while scans are in flight, when the two gicp params disagree on the shared clouds, when front_end is out of
+ * range, and when normals_k changes after the first scan; the previous parameters stay in place */
 int lb_locus_set_params(lb_locus* h, const lb_locus_params* p);
 /* same arguments and blocking rule as lb_odometry_submit; guess = the odometry prior */
 int lb_locus_submit(lb_locus* h, const uint8_t* scan, size_t n_pts, uint32_t point_step, const lb_field* fields,

@@ -78,11 +78,17 @@ class LocusThresholds(C.Structure):
     _fields_ = [("enabled", C.c_int), ("max_translation", C.c_double), ("max_rotation", C.c_double)]
 
 
+class LocusFrontEnd(C.Structure):
+    _fields_ = [("normals_k", C.c_int), ("viewpoint", C.c_float * 3), ("adaptive_voxelization", C.c_int),
+                ("points_to_process", C.c_int)]
+
+
 class LocusParams(C.Structure):
     _fields_ = [("odometry", GicpParams), ("localization", GicpParams), ("odometry_thresholds", LocusThresholds),
                 ("localization_thresholds", LocusThresholds), ("translation_threshold_kf", C.c_double),
                 ("rotation_threshold_kf", C.c_double), ("add_keyframes", C.c_int), ("refresh_every", C.c_int),
-                ("msw", C.c_int), ("window_half_size", C.c_float), ("prior_map", C.c_int), ("initial_pose", C.c_double * 16)]
+                ("msw", C.c_int), ("window_half_size", C.c_float), ("prior_map", C.c_int), ("initial_pose", C.c_double * 16),
+                ("front_end", LocusFrontEnd)]
 
 
 class LocusResult(C.Structure):
@@ -90,7 +96,8 @@ class LocusResult(C.Structure):
                 ("has_odometry", C.c_int), ("odometry", GicpResult), ("odometry_accepted", C.c_int),
                 ("has_localization", C.c_int), ("localization", GicpResult), ("correction_accepted", C.c_int),
                 ("odometry_pose", C.c_double * 16), ("incremental", C.c_double * 16), ("pose", C.c_double * 16),
-                ("keyframe", C.c_int), ("n_inserted", C.c_size_t), ("n_removed", C.c_size_t), ("map_size", C.c_size_t)]
+                ("keyframe", C.c_int), ("n_inserted", C.c_size_t), ("n_removed", C.c_size_t), ("map_size", C.c_size_t),
+                ("leaf_size", C.c_float)]
 
 
 class VoxelInput(C.Structure):
@@ -122,6 +129,7 @@ SYMBOLS = [
     "lb_gicp_set_source_cloud",
     "lb_cloud_release", "lb_gicp_align", "lb_gicp_transform_source", "lb_gicp_nn_target",
     "lb_gicp_fitness", "lb_gicp_point2plane_information", "lb_gicp_compute_normals", "lb_gicp_compute_normals_radius",
+    "lb_gicp_estimate_normals",
     "lb_gicp_statistical_outlier_removal", "lb_gicp_radius_outlier_removal", "lb_gicp_get_covariances", "lb_gicp_cloud_size", "lb_gicp_launch_count",
     "lb_gicp_kernel_time", "lb_gicp_reset_kernel_times",
     "lb_voxel_create", "lb_voxel_create_on_stream", "lb_voxel_destroy", "lb_voxel_set_leaf_size",
@@ -130,9 +138,9 @@ SYMBOLS = [
     "lb_voxel_kernel_time_avg", "lb_voxel_set_input_passthrough", "lb_voxel_filter_merged",
     "lb_features_default_params", "lb_voxel_extract_features",
     "lb_submap_create", "lb_submap_destroy", "lb_submap_clear", "lb_submap_insert", "lb_submap_crop_box", "lb_submap_size",
-    "lb_submap_generation", "lb_submap_points", "lb_submap_neighbors", "lb_submap_launch_count", "lb_gicp_set_target_submap",
+    "lb_submap_generation", "lb_submap_points", "lb_submap_insert_with_normals", "lb_submap_normals", "lb_submap_neighbors", "lb_submap_launch_count", "lb_gicp_set_target_submap",
     "lb_odometry_create", "lb_odometry_destroy", "lb_odometry_voxel", "lb_odometry_gicp", "lb_odometry_depth",
-    "lb_odometry_set_gicp_params", "lb_odometry_set_cloud_sharing", "lb_odometry_submit", "lb_odometry_next", "lb_odometry_pending",
+    "lb_odometry_set_gicp_params", "lb_odometry_set_cloud_sharing", "lb_odometry_set_normals", "lb_odometry_submit", "lb_odometry_next", "lb_odometry_pending",
     "lb_odometry_launch_count", "lb_odometry_stage_times",
     "lb_locus_default_params", "lb_locus_create", "lb_locus_destroy", "lb_locus_voxel", "lb_locus_set_params", "lb_locus_submit",
     "lb_locus_next", "lb_locus_pending", "lb_locus_stage_times",
@@ -199,6 +207,8 @@ def lib():
     L.lb_gicp_get_covariances.argtypes = [vp, i32, vp, sz]
     if hasattr(L, "lb_gicp_compute_normals"):
         L.lb_gicp_compute_normals.argtypes = [vp, i32, i32, vp, vp, i32]
+    if hasattr(L, "lb_gicp_estimate_normals"):
+        L.lb_gicp_estimate_normals.argtypes = [vp, i32, i32, vp]
     if hasattr(L, "lb_gicp_compute_normals_radius"):
         L.lb_gicp_compute_normals_radius.argtypes = [vp, i32, C.c_double, vp, vp, vp, C.POINTER(sz), i32]
     if hasattr(L, "lb_gicp_statistical_outlier_removal"):
@@ -240,6 +250,9 @@ def lib():
         L.lb_submap_size.argtypes = [vp, C.POINTER(sz)]
         L.lb_submap_generation.argtypes = [vp, u64p]
         L.lb_submap_points.argtypes = [vp, vp, sz, i32]
+        if hasattr(L, "lb_submap_normals"):
+            L.lb_submap_insert_with_normals.argtypes = [vp, vp, sz, sz, sz, sz, i32, C.POINTER(sz), vp]
+            L.lb_submap_normals.argtypes = [vp, vp, sz, i32]
         L.lb_submap_neighbors.argtypes = [vp, vp, sz, sz, sz, vp, vp, vp, i32]
         L.lb_submap_launch_count.argtypes = [vp, u64p]
         L.lb_gicp_set_target_submap.argtypes = [vp, vp]
@@ -252,6 +265,8 @@ def lib():
         L.lb_odometry_set_gicp_params.argtypes = [vp, C.POINTER(GicpParams)]
         if hasattr(L, "lb_odometry_set_cloud_sharing"):
             L.lb_odometry_set_cloud_sharing.argtypes = [vp, i32]
+        if hasattr(L, "lb_odometry_set_normals"):
+            L.lb_odometry_set_normals.argtypes = [vp, i32, vp]
         L.lb_odometry_submit.argtypes = [vp, vp, sz, C.c_uint32, C.POINTER(Field), i32, i32, vp, vp, i32, u64p]
         L.lb_odometry_next.argtypes = [vp, C.POINTER(OdometryResult), i32]
         L.lb_odometry_pending.argtypes = [vp, C.POINTER(sz)]
@@ -491,6 +506,12 @@ class GicpB200:
         vp_ = None if viewpoint is None else np.ascontiguousarray(viewpoint, dtype=np.float32)
         _check(lib().lb_gicp_compute_normals(self._h, which, int(k), _ptr(vp_), _ptr(out), LB_MEM_HOST))
         return out
+
+    def estimateNormals(self, which=0, k=20, viewpoint=None):
+        """the same normals written into the source (which=0) or target (which=1) cloud itself: it now has normals, and
+        with recompute_*_covariance = 0 its covariances come from them"""
+        vp_ = None if viewpoint is None else np.ascontiguousarray(viewpoint, dtype=np.float32)
+        _check(lib().lb_gicp_estimate_normals(self._h, which, int(k), _ptr(vp_)))
 
     def computeNormalsRadius(self, which=0, radius=0.3, viewpoint=None):
         """NormalComputation nodelet, radius mode + NaN-normal removal: ((n, 4) float32 normals with NaN rows where a
@@ -743,6 +764,14 @@ class SubmapB200:
         _check(lib().lb_submap_insert(self._h, _ptr(a), a.shape[0], a.shape[1] * 4, 0, LB_MEM_HOST, C.byref(n_ins), _ptr(inc)))
         return (n_ins.value, inc[: n_ins.value]) if want_incremental else n_ins.value
 
+    def InsertPointsWithNormals(self, cloud, normals, want_incremental=False):
+        """cloud, normals: (n, 3) float32, fixed frame; each voxel's winning point keeps its normal"""
+        a = np.ascontiguousarray(np.hstack([np.asarray(cloud, np.float32)[:, :3], np.asarray(normals, np.float32)[:, :3]]))
+        n_ins = C.c_size_t(0)
+        inc = np.zeros((max(len(a), 1), 3), dtype=np.float32) if want_incremental else None
+        _check(lib().lb_submap_insert_with_normals(self._h, _ptr(a), a.shape[0], 24, 0, 12, LB_MEM_HOST, C.byref(n_ins), _ptr(inc)))
+        return (n_ins.value, inc[: n_ins.value]) if want_incremental else n_ins.value
+
     def insert_device(self, ptr, n, stride, xyz_off=0):
         n_ins = C.c_size_t(0)
         _check(lib().lb_submap_insert(self._h, C.c_void_p(int(ptr)), n, stride, xyz_off, LB_MEM_DEVICE, C.byref(n_ins), None))
@@ -768,6 +797,12 @@ class SubmapB200:
     def points(self):
         out = np.zeros((self.size(), 3), dtype=np.float32)
         _check(lib().lb_submap_points(self._h, _ptr(out), out.shape[0], LB_MEM_HOST))
+        return out
+
+    def normals(self):
+        """(n, 3) float32 in insertion order; NaN rows for points inserted without a normal"""
+        out = np.zeros((self.size(), 3), dtype=np.float32)
+        _check(lib().lb_submap_normals(self._h, _ptr(out), out.shape[0], LB_MEM_HOST))
         return out
 
     def ApproxNearestNeighbors(self, cloud):
@@ -833,6 +868,11 @@ class OdometryB200:
         """each scan's index + covariances computed once and adopted as the next registration's target (idle pipeline only)"""
         _check(lib().lb_odometry_set_cloud_sharing(self._h, int(bool(on))))
 
+    def setNormals(self, k=20, viewpoint=None):
+        """normals stage: every filtered scan gets its k-NN normals (k = 0: off); idle pipeline, before the first scan"""
+        vp_ = None if viewpoint is None else np.ascontiguousarray(viewpoint, dtype=np.float32)
+        _check(lib().lb_odometry_set_normals(self._h, int(k), _ptr(vp_)))
+
     def submit(self, scan, n_pts, point_step, fields, mem=LB_MEM_HOST, guess=None, filtered_out=None,
                mem_filtered=LB_MEM_HOST):
         """scan / filtered_out: host uint8 numpy arrays or raw pointers (int).  Returns the ticket."""
@@ -874,7 +914,7 @@ class OdometryB200:
 
 def locus_params(**kw):
     """lb_locus_params with the reference's shipped values; keywords override top-level fields, and `odometry` /
-    `localization` / `*_thresholds` take dicts of their fields"""
+    `localization` / `*_thresholds` / `front_end` take dicts of their fields"""
     p = LocusParams()
     _check(lib().lb_locus_default_params(C.byref(p)))
     for k, v in kw.items():
@@ -885,7 +925,10 @@ def locus_params(**kw):
             for kk, vv in v.items():
                 if not hasattr(sub, kk):
                     raise AttributeError("%s.%s" % (k, kk))
-                setattr(sub, kk, vv)
+                if kk == "viewpoint":
+                    sub.viewpoint[:] = [float(x) for x in np.asarray(vv, dtype=np.float32).reshape(3)]
+                else:
+                    setattr(sub, kk, vv)
         elif k == "initial_pose":
             p.initial_pose[:] = [float(x) for x in np.asarray(v, dtype=np.float64).reshape(16)]
         else:

@@ -1441,6 +1441,52 @@ int lb_gicp_compute_normals(lb_gicp* h, int which, int k, const float* viewpoint
   return LB_OK;
 }
 
+// The same kernels with the cloud's own normal buffer as output: NormalFin writes (nx, ny, nz, curvature) in original
+// order, which is Cloud::nrm's layout (the covariance and transform kernels read x, y, z only).  Asynchronous: the
+// source's consumers run on the handle's stream, the target's on stream2 (joined into the handle's stream here).
+int lb_gicp_estimate_normals(lb_gicp* h, int which, int k, const float* viewpoint) {
+  if (!h || (which != 0 && which != 1)) { set_error("lb_gicp_estimate_normals: bad argument"); return LB_ERR_INVALID_ARG; }
+  std::shared_ptr<Cloud>& ref = which == 0 ? h->src : h->tgt;
+  Cloud& cl = *ref;
+  if (!cl.valid) { set_error("lb_gicp_estimate_normals: no %s cloud", which == 0 ? "source" : "target"); return which == 0 ? LB_ERR_EMPTY_SOURCE : LB_ERR_NO_TARGET; }
+  if (k < 3 || k > 20) { set_error("lb_gicp_estimate_normals: k must be in [3, 20] (PCL yields NaN normals below 3)"); return LB_ERR_UNSUPPORTED; }
+  if ((size_t)k > cl.n) { set_error("lb_gicp_estimate_normals: cloud has %zu points, fewer than k = %d", cl.n, k); return LB_ERR_TOO_FEW_POINTS; }
+  // a target adopted from this handle's previous source is held twice by the handle itself; any other holder means the
+  // cloud was shared (or adopted from another handle) and is immutable
+  const long own_refs = 1 + (h->last_src == ref ? 1 : 0);
+  if (ref->owner != h || ref.use_count() > own_refs) {
+    set_error("lb_gicp_estimate_normals: the %s cloud is shared with another handle", which == 0 ? "source" : "target");
+    return LB_ERR_INVALID_ARG;
+  }
+  Scratch& S = h->sc[which];
+  Ctx& c = S.c;
+  LB_CUDA(cudaSetDevice(c.device));
+  const size_t cap = cl.n > h->max_points_seen[which] ? cl.n : h->max_points_seen[which];
+  LB_TRY(cl.nrm.ensure(cap));
+  LB_TRY(finish_index(h, cl, which));
+  const uint32_t N = (uint32_t)cl.n;
+  LB_TRY(S.worklist.ensure(N));
+  uint32_t* d_wl = S.d_u32 + 4;
+  LB_CUDA(cudaMemsetAsync(d_wl, 0, 2 * sizeof(uint32_t), c.stream));
+  NormalFin fin;
+  fin.vp[0] = viewpoint ? viewpoint[0] : 0.f; fin.vp[1] = viewpoint ? viewpoint[1] : 0.f; fin.vp[2] = viewpoint ? viewpoint[2] : 0.f;
+  fin.out = cl.nrm.p;
+  GridView v = cl.view();
+  static const int ring_cap = [] { const char* e = getenv("LB_RING_CAP"); return e ? atoi(e) : 6; }();
+  knn_cov_quadreg_kernel<20, NormalFin><<<cdiv(4ll * N, KQ_THREADS), KQ_THREADS, 0, c.stream>>>(v, cl.raw.p, k, fin, 99, ring_cap,
+                                                                                        S.worklist.p, d_wl, nullptr);
+  knn_cov_tail_kernel<20, NormalFin><<<c.sm_count * 2, 128, 0, c.stream>>>(v, k, fin, S.worklist.p, d_wl);
+  c.launches += 2;
+  LB_CUDA(cudaGetLastError());
+  if (which == 1) {
+    LB_CUDA(cudaEventRecord(h->ev_join, c.stream));
+    LB_CUDA(cudaStreamWaitEvent(h->c.stream, h->ev_join, 0));
+  }
+  cl.has_normals = true;
+  cl.cov_valid = false;
+  return LB_OK;
+}
+
 // SURVEY 8f row f2, the nodelet's radius mode + NaN-normal removal (normal_computation.cc:53-57,73-77).
 int lb_gicp_compute_normals_radius(lb_gicp* h, int which, double radius, const float* viewpoint, float* out4, int32_t* valid_idx,
                                    size_t* n_valid, int mem) {

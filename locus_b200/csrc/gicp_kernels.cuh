@@ -2112,13 +2112,19 @@ sm_decide_kernel(const uint32_t* __restrict__ slot_of, const uint32_t* __restric
 __global__ void __launch_bounds__(256)
 sm_commit_kernel(const uint8_t* __restrict__ base, uint32_t n, uint32_t stride, uint32_t xyz_off, const uint32_t* __restrict__ slot_of,
                  const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t n_old, f4* __restrict__ pts,
-                 uint32_t* __restrict__ owner, float* __restrict__ inserted_xyz /*nullable*/) {
+                 uint32_t* __restrict__ owner, float* __restrict__ inserted_xyz /*nullable*/, int normal_off,
+                 f4* __restrict__ nrm /*nullable: the map keeps no normals yet*/) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n || !flags[i]) return;
   const float* p = reinterpret_cast<const float*>(base + (size_t)i * stride + xyz_off);
   const uint32_t j = n_old + pos[i];
   pts[j] = f4{p[0], p[1], p[2], 1.0f};
   owner[slot_of[i]] = j;
+  if (nrm) {
+    // a point inserted without a normal: all four words NaN (w = 0 marks a stored normal)
+    const float* m = reinterpret_cast<const float*>(base + (size_t)i * stride + (normal_off >= 0 ? normal_off : 0));
+    nrm[j] = normal_off >= 0 ? f4{m[0], m[1], m[2], 0.0f} : f4{__int_as_float(-1), __int_as_float(-1), __int_as_float(-1), __int_as_float(-1)};
+  }
   if (inserted_xyz) { inserted_xyz[3 * (size_t)pos[i]] = p[0]; inserted_xyz[3 * (size_t)pos[i] + 1] = p[1]; inserted_xyz[3 * (size_t)pos[i] + 2] = p[2]; }
 }
 
@@ -2148,11 +2154,17 @@ sm_crop_flags_kernel(const f4* __restrict__ pts, uint32_t n, float cx, float cy,
 __global__ void __launch_bounds__(256)
 sm_compact_kernel(const f4* __restrict__ pts, const double* __restrict__ cov, uint32_t n, uint32_t n_cov,
                   const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, f4* __restrict__ pts_out,
-                  double* __restrict__ cov_out) {
+                  double* __restrict__ cov_out, const f4* __restrict__ nrm /*nullable*/, f4* __restrict__ nrm_out,
+                  uint32_t* __restrict__ n_plain /*nullable: counts the survivors without a normal*/) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n || !flags[j]) return;
   const uint32_t d = pos[j];
   pts_out[d] = pts[j];
+  if (nrm) {
+    const f4 m = nrm[j];
+    nrm_out[d] = m;
+    if (n_plain && m.w != m.w) atomicAdd(n_plain, 1u);     // w: 0 with a normal (which may itself be NaN), NaN without
+  }
   if (j < n_cov) {
 #pragma unroll
     for (int e = 0; e < 6; e++) cov_out[6 * (size_t)d + e] = cov[6 * (size_t)j + e];

@@ -17,6 +17,7 @@
 // bound to the caller's lb_submap, localizing the scans strictly in order (pose semantics: lo_pose.h).  In that mode a
 // ticket is done when stage L has finished it, so stages V and G run at most the usual in-flight bound ahead of it.
 #include <chrono>
+#include <cmath>
 #include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
@@ -28,8 +29,10 @@
 
 #if defined(LB_LOCUS_STUB)       // TEST-ONLY build without CUDA: tests/locus_harness.cpp supplies fake stages
 #include "locus_stub.h"
+#include "front_end_stub.h"
 #elif defined(LB_ODOMETRY_STUB)  // TEST-ONLY build without CUDA: tests/odometry_harness.cpp supplies fake stages
 #include "odometry_stub.h"
+#include "front_end_stub.h"
 #else
 #include "prims.cuh"
 #endif
@@ -73,6 +76,7 @@ struct Entry {           // per in-flight ticket
   lb_odometry_result res;
   bool filtered = false; // stage V done
   bool aligned = false;  // stage G done (lb_locus only)
+  float leaf = 0.f;      // lb_locus: the VoxelGrid x leaf the scan was filtered with
   bool done = false;     // result complete: stage G done, or stage L with lb_locus
   lb_cloud* loc_cloud = nullptr;   // lb_locus: stage L's reference to this scan's prepared cloud
   lb_locus_result loc;             // lb_locus: filled by stage L
@@ -91,6 +95,15 @@ struct lb_odometry {
   std::vector<Prepared> prep;          // same indexing as ring (ticket % R); used when share is on
   bool share = true;                   // lb_odometry_set_cloud_sharing (on by default)
   bool chain = false;                  // run by lb_locus: stage L completes the tickets
+  int normals_k = 0;                   // lb_odometry_set_normals (0 = off)
+  float normals_vp[3] = {0.f, 0.f, 0.f};
+  // lb_locus's adaptive input voxelization (Locus.cc:780-810), touched by stage V only (and by lb_locus_set_params
+  // while nothing is in flight)
+  bool adaptive = false;
+  int points_to_process = 0;
+  bool leaf_started = false;           // `leaf` holds the VoxelGrid's leaf as of the first scan
+  double leaf = 0;                     // double_param.value
+  int leaf_counter = 0;                // counter_voxel_
   cudaStream_t copy_stream = nullptr;
   cudaStream_t voxel_stream = nullptr;
 
@@ -129,6 +142,20 @@ void advance_done_floor(lb_odometry* h) {   // mu held
   }
 }
 
+// Locus::ApplyAdaptiveInputVoxelization (Locus.cc:780-810) after a scan whose VoxelGrid kept n points.  The reference
+// publishes the new leaf on a topic and the VoxelGrid nodelet applies it to whichever scan it filters next; here it
+// applies to the next scan exactly (the same rule, deterministic timing).
+void adapt_leaf(lb_odometry* h, size_t n) {
+  double d = h->leaf * ((double)n / (double)h->points_to_process);
+  if (d < 0.01) d = 0.01;
+  if (d > 5.0) d = 5.0;
+  const bool change = std::abs(h->leaf - d) > 0.01 || h->leaf_counter % 20 == 0;
+  if (change) { h->leaf = d; h->leaf_counter = 0; }
+  h->leaf_counter++;
+  // CustomVoxelGrid::ChangeLeafSizeRostopic (custom_voxel_grid.cc:62-73): the double becomes a float leaf on every axis
+  if (change) lb_voxel_set_leaf_size(h->vg, (float)h->leaf, (float)h->leaf, (float)h->leaf);
+}
+
 void voxel_stage(lb_odometry* h) {
   cudaSetDevice(h->device);
   const uint64_t R = h->ring.size();
@@ -150,10 +177,16 @@ void voxel_stage(lb_odometry* h) {
     Slot& s = h->ring[t % R];
     const Job& j = e->job;
     size_t n_out = 0;
+    float leaf3[3] = {0.f, 0.f, 0.f};
+    if (h->chain) {
+      lb_voxel_get_leaf_size(h->vg, leaf3);
+      if (!h->leaf_started) { h->leaf = leaf3[0]; h->leaf_started = true; }
+    }
     int st = lb_voxel_filter(h->vg, j.scan, j.n_pts, j.point_step, j.fields.data(), (int)j.fields.size(), nullptr, 0, s.d,
                              h->max_points, &n_out, nullptr, j.mem, LB_MEM_DEVICE);
     s.status = st; s.n = (st == LB_OK) ? n_out : 0; s.point_step = j.point_step; s.xyz_off = j.xyz_off;
     if (st != LB_OK) copy_err(s.error, sizeof(s.error));
+    if (st == LB_OK && h->adaptive) adapt_leaf(h, n_out);     // a failed VoxelGrid is a callback that never ran
     if (st == LB_OK && j.filtered_out && n_out) {
       cudaError_t ce = cudaMemcpyAsync(j.filtered_out, s.d, n_out * j.point_step,
                                        j.mem_filtered == LB_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice,
@@ -168,6 +201,7 @@ void voxel_stage(lb_odometry* h) {
       std::lock_guard<std::mutex> lk(h->mu);
       e->filtered = true;
       e->res.n_filtered = s.n;
+      e->leaf = leaf3[0];
       h->next_filter = t + 1;
       h->t_voxel_wait += std::chrono::duration<double>(tb0 - tw0).count();
       h->t_voxel_busy += std::chrono::duration<double>(std::chrono::steady_clock::now() - tb0).count();
@@ -203,6 +237,7 @@ void align_stage(lb_odometry* h, int w) {
       int st = cur.status;
       if (st == LB_OK && cur.n > 0) {
         st = lb_gicp_set_source(g, cur.d, cur.n, cur.point_step, (size_t)cur.xyz_off, LB_NO_NORMALS, LB_MEM_DEVICE);
+        if (st == LB_OK && h->normals_k) st = lb_gicp_estimate_normals(g, 0, h->normals_k, h->normals_vp);
         if (st == LB_OK) st = lb_gicp_prepare_source(g);
         if (st == LB_OK) st = lb_gicp_share_source(g, &mine);
         // the chain's stage L adopts the same cloud as its localization source: its reference, not the ring slot,
@@ -241,8 +276,10 @@ void align_stage(lb_odometry* h, int w) {
       const Slot& prv = h->ring[(t - 1) % R];
       if (prv.status == LB_OK && prv.n > 0 && cur.n > 0) {
         int st = lb_gicp_set_source(g, cur.d, cur.n, cur.point_step, (size_t)cur.xyz_off, LB_NO_NORMALS, LB_MEM_DEVICE);
+        if (st == LB_OK && h->normals_k) st = lb_gicp_estimate_normals(g, 0, h->normals_k, h->normals_vp);
         if (st == LB_OK)
           st = lb_gicp_set_target(g, prv.d, prv.n, prv.point_step, (size_t)prv.xyz_off, LB_NO_NORMALS, LB_MEM_DEVICE, nullptr);
+        if (st == LB_OK && h->normals_k) st = lb_gicp_estimate_normals(g, 1, h->normals_k, h->normals_vp);
         if (st == LB_OK) st = lb_gicp_align(g, e->job.has_guess ? e->job.guess : nullptr, &r.gicp);
         r.status = st;
         if (st == LB_OK) r.has_pose = 1; else copy_err(r.error, sizeof(r.error));
@@ -400,6 +437,22 @@ int lb_odometry_set_cloud_sharing(lb_odometry* h, int on) {
   return LB_OK;
 }
 
+int lb_odometry_set_normals(lb_odometry* h, int k, const float* viewpoint) {
+  if (!h) { set_error("lb_odometry_set_normals: null handle"); return LB_ERR_INVALID_ARG; }
+  if (k != 0 && (k < 3 || k > 20)) { set_error("lb_odometry_set_normals: k must be 0 (off) or in [3, 20]"); return LB_ERR_UNSUPPORTED; }
+  const float vp[3] = {viewpoint ? viewpoint[0] : 0.f, viewpoint ? viewpoint[1] : 0.f, viewpoint ? viewpoint[2] : 0.f};
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (h->next_return != h->next_ticket) { set_error("lb_odometry_set_normals: pipeline not idle"); return LB_ERR_INVALID_ARG; }
+  if (h->next_ticket != 0 && (k != h->normals_k || memcmp(vp, h->normals_vp, sizeof(vp)) != 0)) {
+    // the previous scan's prepared cloud was built with the old setting
+    set_error("lb_odometry_set_normals: change before the first scan is submitted");
+    return LB_ERR_UNSUPPORTED;
+  }
+  h->normals_k = k;
+  memcpy(h->normals_vp, vp, sizeof(vp));
+  return LB_OK;
+}
+
 int lb_odometry_submit(lb_odometry* h, const uint8_t* scan, size_t n_pts, uint32_t point_step, const lb_field* fields,
                        int n_fields, int mem, const float* guess, uint8_t* filtered_out, int mem_filtered,
                        uint64_t* ticket) {
@@ -483,8 +536,8 @@ struct lb_locus {
   lb_odometry* core = nullptr;
   lb_gicp* g = nullptr;            // stage L's handle (own stream); source = the shared cloud, target = the submap
   lb_submap* map = nullptr;        // the caller's
-  float* d_xyz = nullptr;          // a keyframe's points in the fixed frame, max_points x 3 floats
-  lb_locus_params P;
+  float* d_xyz = nullptr;          // a keyframe's points in the fixed frame, max_points x 6 floats (xyz, normal)
+  lb_locus_params P{};
   // pose state, touched by stage L only (and by set_params while nothing is in flight)
   bool started = false;            // the first scan has been taken
   lo::Pose O, L, KF;               // odometry estimate, localization estimate, last keyframe
@@ -499,9 +552,15 @@ namespace {
 int locus_insert(lb_locus* c, size_t n, lb_locus_result& r) {
   float T[16];
   lo::to_mat(c->L, T);
-  LB_TRY(lb_gicp_transform_source(c->g, T, c->d_xyz, 12, 0, LB_NO_NORMALS, LB_MEM_DEVICE));
   size_t ins = 0;
-  LB_TRY(lb_submap_insert(c->map, c->d_xyz, n, 12, 0, LB_MEM_DEVICE, &ins, nullptr));
+  if (c->P.front_end.normals_k) {
+    // Locus.cc:530-532: the keyframe enters the map with its normals rotated into the fixed frame
+    LB_TRY(lb_gicp_transform_source(c->g, T, c->d_xyz, 24, 0, 12, LB_MEM_DEVICE));
+    LB_TRY(lb_submap_insert_with_normals(c->map, c->d_xyz, n, 24, 0, 12, LB_MEM_DEVICE, &ins, nullptr));
+  } else {
+    LB_TRY(lb_gicp_transform_source(c->g, T, c->d_xyz, 12, 0, LB_NO_NORMALS, LB_MEM_DEVICE));
+    LB_TRY(lb_submap_insert(c->map, c->d_xyz, n, 12, 0, LB_MEM_DEVICE, &ins, nullptr));
+  }
   r.keyframe = 1;
   r.n_inserted = ins;
   return LB_OK;
@@ -540,7 +599,7 @@ void locus_scan(lb_locus* c, Entry* e) {
   const lb_odometry_result& o = e->res;
   lb_locus_result& r = e->loc;
   memset(&r, 0, sizeof(r));
-  r.ticket = o.ticket; r.status = o.status; r.n_filtered = o.n_filtered;
+  r.ticket = o.ticket; r.status = o.status; r.n_filtered = o.n_filtered; r.leaf_size = e->leaf;
   memcpy(r.error, o.error, sizeof(r.error));
   r.has_odometry = o.has_pose;
   r.odometry = o.gicp;
@@ -610,15 +669,36 @@ int locus_apply_params(lb_locus* c, const lb_locus_params* p) {
               "index_cell_size (each scan's index and covariances are built once for both)");
     return LB_ERR_INVALID_ARG;
   }
+  if (p->odometry.recompute_source_covariance != p->odometry.recompute_target_covariance ||
+      p->odometry.recompute_source_covariance != p->localization.recompute_source_covariance) {
+    set_error("lb_locus_set_params: the odometry's recompute_source_covariance and recompute_target_covariance and the "
+              "localization's recompute_source_covariance must agree (one prepared cloud serves all three)");
+    return LB_ERR_INVALID_ARG;
+  }
   if (p->refresh_every < 1 || !(p->window_half_size > 0.f)) {
     set_error("lb_locus_set_params: need refresh_every >= 1 and window_half_size > 0");
     return LB_ERR_INVALID_ARG;
   }
-  LB_TRY(lb_gicp_set_params(c->g, &p->localization));
-  int st = lb_odometry_set_gicp_params(c->core, &p->odometry);
+  const lb_locus_front_end& fe = p->front_end;
+  if ((fe.normals_k != 0 && (fe.normals_k < 3 || fe.normals_k > 20)) || (fe.adaptive_voxelization && fe.points_to_process <= 0)) {
+    set_error("lb_locus_set_params: front_end needs normals_k = 0 or in [3, 20], and points_to_process > 0 with "
+              "adaptive_voxelization");
+    return LB_ERR_INVALID_ARG;
+  }
+  LB_TRY(lb_odometry_set_normals(c->core, fe.normals_k, fe.viewpoint));
+  int st = lb_gicp_set_params(c->g, &p->localization);
+  if (st == LB_OK) {
+    st = lb_odometry_set_gicp_params(c->core, &p->odometry);
+    if (st != LB_OK) lb_gicp_set_params(c->g, &c->P.localization);   // keep the previous state
+  }
   if (st != LB_OK) {
-    lb_gicp_set_params(c->g, &c->P.localization);   // keep the previous state
+    lb_odometry_set_normals(c->core, c->P.front_end.normals_k, c->P.front_end.viewpoint);
     return st;
+  }
+  {
+    std::lock_guard<std::mutex> lk(c->core->mu);
+    c->core->adaptive = fe.adaptive_voxelization != 0;
+    c->core->points_to_process = fe.points_to_process;
   }
   c->P = *p;
   if (!c->started) {
@@ -671,12 +751,12 @@ int lb_locus_create(int device, int depth, size_t max_points, uint32_t max_point
   }
   lb_locus* c = new lb_locus;
   c->map = map;
-  lb_locus_params P;
+  lb_locus_params P{};
   lb_locus_default_params(&P);
   int st = odometry_create(device, depth, max_points, max_point_step, true, &c->core);
   if (st == LB_OK) st = lb_gicp_create(device, &c->g);
   if (st == LB_OK) st = lb_gicp_reserve(c->g, max_points, 0);
-  if (st == LB_OK && cudaMalloc((void**)&c->d_xyz, max_points * 3 * sizeof(float)) != cudaSuccess) {
+  if (st == LB_OK && cudaMalloc((void**)&c->d_xyz, max_points * 6 * sizeof(float)) != cudaSuccess) {
     set_error("lb_locus_create: allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
     st = LB_ERR_CUDA;
   }

@@ -17,6 +17,8 @@
 // unpinned": here a voxel is world-anchored (floor(p / resolution)), and "approximate nearest" is exact nearest.
 // oracle/submap_oracle.py restates exactly these semantics on the CPU for the tests.
 #pragma once
+#include <algorithm>
+#include <limits>
 
 struct lb_submap {
   lb_gicp* eng = nullptr;              // index / k-NN engine (its stream orders all submap work)
@@ -26,6 +28,12 @@ struct lb_submap {
   int cov_k = 0; double cov_eps = 0;   // parameters the cache was computed with
   DBuf<f4> pts[2];                     // ping-pong (crop compacts into the other one)
   DBuf<double> cov[2];                 // covariance cache, insertion order, 6 per point
+  DBuf<f4> nrm[2];                     // normals paired with pts[] (from the first insert with normals on): w = 0 with
+                                       // a normal, every word NaN without one
+  bool nrm_on = false;
+  size_t n_plain = 0;                  // map points inserted without a normal
+  bool cov_from_normals = false;       // the engine cloud's covariances came from the normals ...
+  double nrm_cov_eps = 0;              // ... with this gicp_epsilon
   int cur = 0;
   DBuf<unsigned long long> keys;       // occupancy hash
   DBuf<uint32_t> owner;
@@ -34,7 +42,7 @@ struct lb_submap {
   DBuf<uint8_t> stage;
   DBuf<int32_t> nn_idx; DBuf<float> nn_d2; DBuf<float> out_xyz;
   ScanWork scan;
-  uint32_t* d_count = nullptr; uint32_t* h_count = nullptr;
+  uint32_t* d_count = nullptr; uint32_t* h_count = nullptr;   // [0] scan totals, [1] crop survivors without a normal
   uint64_t generation = 0;             // bumps on every change of the point set
   uint64_t indexed_generation = ~0ull; // generation the engine's cloud was built from
 };
@@ -84,6 +92,8 @@ int submap_ensure_index(lb_submap* m) {
   return LB_OK;
 }
 
+int submap_adopt(lb_gicp* h, lb_submap* m);
+
 }  // namespace
 
 extern "C" {
@@ -95,7 +105,7 @@ int lb_submap_create(int device, float resolution, lb_submap** out) {
   int s = lb_gicp_create(device, &m->eng);
   if (s != LB_OK) { delete m; return s; }
   m->res = resolution;
-  if (cudaMalloc((void**)&m->d_count, sizeof(uint32_t)) != cudaSuccess || cudaMallocHost((void**)&m->h_count, sizeof(uint32_t)) != cudaSuccess) {
+  if (cudaMalloc((void**)&m->d_count, 2 * sizeof(uint32_t)) != cudaSuccess || cudaMallocHost((void**)&m->h_count, 2 * sizeof(uint32_t)) != cudaSuccess) {
     set_error("lb_submap_create: allocation failed");
     lb_gicp_destroy(m->eng); delete m;
     return LB_ERR_CUDA;
@@ -110,7 +120,7 @@ int lb_submap_destroy(lb_submap* m) {
   if (!m) return LB_OK;
   cudaSetDevice(m->eng->c.device);
   cudaStreamSynchronize(m->eng->c.stream);
-  for (int i = 0; i < 2; i++) { m->pts[i].release(); m->cov[i].release(); }
+  for (int i = 0; i < 2; i++) { m->pts[i].release(); m->cov[i].release(); m->nrm[i].release(); }
   m->keys.release(); m->owner.release(); m->slot_of.release(); m->flags.release(); m->pos.release(); m->stage.release();
   m->nn_idx.release(); m->nn_d2.release(); m->out_xyz.release(); m->scan.sums.release();
   if (m->d_count) cudaFree(m->d_count);
@@ -135,18 +145,26 @@ int lb_submap_generation(lb_submap* m, uint64_t* g) {
 int lb_submap_clear(lb_submap* m) {
   if (!m) return LB_ERR_INVALID_ARG;
   LB_CUDA(cudaSetDevice(m->eng->c.device));
-  m->n = 0; m->n_cov = 0; m->generation++;
+  m->n = 0; m->n_cov = 0; m->n_plain = 0; m->generation++;
   return submap_rehash(m, 1u << 16);
 }
 
-int lb_submap_insert(lb_submap* m, const void* pts, size_t n, size_t stride, size_t xyz_off, int mem, size_t* n_inserted,
-                     float* inserted_xyz) {
-  if (!m) { set_error("lb_submap_insert: null handle"); return LB_ERR_INVALID_ARG; }
+}  // extern "C"
+
+namespace {
+
+// lb_submap_insert (normal_off < 0) and lb_submap_insert_with_normals
+int submap_insert(lb_submap* m, const void* pts, size_t n, size_t stride, size_t xyz_off, ptrdiff_t normal_off, int mem,
+                  size_t* n_inserted, float* inserted_xyz, const char* who) {
+  if (!m) { set_error("%s: null handle", who); return LB_ERR_INVALID_ARG; }
   if (n_inserted) *n_inserted = 0;
   if (n == 0) return LB_OK;
-  if (!pts) { set_error("lb_submap_insert: null cloud"); return LB_ERR_INVALID_ARG; }
-  if ((stride & 3u) || (xyz_off & 3u) || xyz_off + 12 > stride) { set_error("lb_submap_insert: bad stride/offset"); return LB_ERR_INVALID_ARG; }
-  if (m->n + n > 0x7ffffff0ull) { set_error("lb_submap_insert: too many points"); return LB_ERR_INVALID_ARG; }
+  if (!pts) { set_error("%s: null cloud", who); return LB_ERR_INVALID_ARG; }
+  if ((stride & 3u) || (xyz_off & 3u) || xyz_off + 12 > stride || (normal_off >= 0 && ((normal_off & 3) || (size_t)normal_off + 12 > stride))) {
+    set_error("%s: bad stride/offset", who);
+    return LB_ERR_INVALID_ARG;
+  }
+  if (m->n + n > 0x7ffffff0ull) { set_error("%s: too many points", who); return LB_ERR_INVALID_ARG; }
   Ctx& c = m->eng->c;
   LB_CUDA(cudaSetDevice(c.device));
   const uint32_t N = (uint32_t)n;
@@ -158,6 +176,13 @@ int lb_submap_insert(lb_submap* m, const void* pts, size_t n, size_t stride, siz
   }
   // room for every candidate: points, and a table that stays at most half full
   LB_TRY(grow_preserving(m->pts[m->cur], m->n + n, m->n, c.stream));
+  if (normal_off >= 0 && !m->nrm_on) {
+    // the first insert with normals: the points already in the map have none
+    LB_TRY(grow_preserving(m->nrm[m->cur], m->n + n, 0, c.stream));
+    if (m->n) LB_CUDA(cudaMemsetAsync(m->nrm[m->cur].p, 0xff, m->n * sizeof(f4), c.stream));
+    m->nrm_on = true;
+  }
+  if (m->nrm_on) LB_TRY(grow_preserving(m->nrm[m->cur], m->n + n, m->n, c.stream));
   if ((m->n + n) * 2 > m->cap) LB_TRY(submap_rehash(m, (uint32_t)((m->n + n) * 2 + 1)));
   LB_TRY(m->slot_of.ensure(n)); LB_TRY(m->flags.ensure(n)); LB_TRY(m->pos.ensure(n));
   float* d_ins = nullptr;
@@ -170,7 +195,8 @@ int lb_submap_insert(lb_submap* m, const void* pts, size_t n, size_t stride, siz
   c.launches += 2;
   LB_TRY(exclusive_scan_u32(c, m->scan, m->flags.p, m->pos.p, n, m->d_count));
   sm_commit_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(d_src, N, (uint32_t)stride, (uint32_t)xyz_off, m->slot_of.p, m->flags.p, m->pos.p,
-                                                       (uint32_t)m->n, m->pts[m->cur].p, m->owner.p, d_ins);
+                                                       (uint32_t)m->n, m->pts[m->cur].p, m->owner.p, d_ins, (int)normal_off,
+                                                       m->nrm_on ? m->nrm[m->cur].p : nullptr);
   c.launches++;
   LB_CUDA(cudaMemcpyAsync(m->h_count, m->d_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
   LB_CUDA(cudaStreamSynchronize(c.stream));
@@ -181,8 +207,24 @@ int lb_submap_insert(lb_submap* m, const void* pts, size_t n, size_t stride, siz
     LB_CUDA(cudaStreamSynchronize(c.stream));
   }
   if (added) { m->n += added; m->generation++; }
+  if (normal_off < 0) m->n_plain += added;
   if (n_inserted) *n_inserted = added;
   return LB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int lb_submap_insert(lb_submap* m, const void* pts, size_t n, size_t stride, size_t xyz_off, int mem, size_t* n_inserted,
+                     float* inserted_xyz) {
+  return submap_insert(m, pts, n, stride, xyz_off, -1, mem, n_inserted, inserted_xyz, "lb_submap_insert");
+}
+
+int lb_submap_insert_with_normals(lb_submap* m, const void* pts, size_t n, size_t stride, size_t xyz_off, size_t normal_off,
+                                  int mem, size_t* n_inserted, float* inserted_xyz) {
+  if (normal_off > 0x7fffffffull) { set_error("lb_submap_insert_with_normals: bad normal offset"); return LB_ERR_INVALID_ARG; }
+  return submap_insert(m, pts, n, stride, xyz_off, (ptrdiff_t)normal_off, mem, n_inserted, inserted_xyz, "lb_submap_insert_with_normals");
 }
 
 int lb_submap_crop_box(lb_submap* m, const float* center3, float half_size, size_t* n_removed) {
@@ -196,17 +238,24 @@ int lb_submap_crop_box(lb_submap* m, const float* center3, float half_size, size
   LB_TRY(m->flags.ensure(m->n)); LB_TRY(m->pos.ensure(m->n));
   LB_TRY(m->pts[o].ensure(m->pts[m->cur].cap));
   if (m->n_cov) LB_TRY(m->cov[o].ensure(6 * m->n_cov));
+  if (m->nrm_on) LB_TRY(m->nrm[o].ensure(m->nrm[m->cur].cap));
+  // survivors without a normal: counted only when the map mixes points with and without one
+  const bool count_plain = m->nrm_on && m->n_plain > 0 && m->n_plain < m->n;
+  if (count_plain) LB_CUDA(cudaMemsetAsync(m->d_count + 1, 0, sizeof(uint32_t), c.stream));
   sm_crop_flags_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(m->pts[m->cur].p, N, center3[0], center3[1], center3[2], half_size, m->flags.p);
   c.launches++;
   LB_TRY(exclusive_scan_u32(c, m->scan, m->flags.p, m->pos.p, m->n, m->d_count));
   sm_compact_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(m->pts[m->cur].p, m->n_cov ? m->cov[m->cur].p : nullptr, N, (uint32_t)m->n_cov,
-                                                        m->flags.p, m->pos.p, m->pts[o].p, m->n_cov ? m->cov[o].p : nullptr);
+                                                        m->flags.p, m->pos.p, m->pts[o].p, m->n_cov ? m->cov[o].p : nullptr,
+                                                        m->nrm_on ? m->nrm[m->cur].p : nullptr, m->nrm_on ? m->nrm[o].p : nullptr,
+                                                        count_plain ? m->d_count + 1 : nullptr);
   c.launches++;
   // survivors among the points that had a cached covariance: they stay a prefix (the compaction is stable)
   uint32_t* h2 = m->h_count;
-  LB_CUDA(cudaMemcpyAsync(h2, m->d_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+  LB_CUDA(cudaMemcpyAsync(h2, m->d_count, (count_plain ? 2 : 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
   LB_CUDA(cudaStreamSynchronize(c.stream));
-  const size_t kept = *h2;
+  const size_t kept = h2[0];
+  const size_t kept_plain = m->n_plain == 0 ? 0 : (count_plain ? h2[1] : kept);
   size_t kept_cov = 0;
   if (m->n_cov) {
     if (m->n_cov == m->n) kept_cov = kept;
@@ -219,7 +268,7 @@ int lb_submap_crop_box(lb_submap* m, const float* center3, float half_size, size
   }
   if (n_removed) *n_removed = m->n - kept;
   if (kept == m->n) return LB_OK;                 // nothing left the window
-  m->cur = o; m->n = kept; m->n_cov = kept_cov; m->generation++;
+  m->cur = o; m->n = kept; m->n_cov = kept_cov; m->n_plain = kept_plain; m->generation++;
   return submap_rehash(m, (uint32_t)(kept * 2 + 1));
 }
 
@@ -236,6 +285,32 @@ int lb_submap_points(lb_submap* m, float* xyz_out, size_t capacity_points, int m
   LB_TRY(m->nn_idx.ensure(m->n));
   iota_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(m->nn_idx.p, N);
   sm_gather_xyz_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(m->pts[m->cur].p, m->nn_idx.p, N, d);
+  c.launches += 2;
+  if (mem == LB_MEM_HOST) LB_CUDA(cudaMemcpyAsync(xyz_out, d, 3 * m->n * sizeof(float), cudaMemcpyDeviceToHost, c.stream));
+  LB_CUDA(cudaStreamSynchronize(c.stream));
+  return LB_OK;
+}
+
+int lb_submap_normals(lb_submap* m, float* xyz_out, size_t capacity_points, int mem) {
+  if (!m || !xyz_out) { set_error("lb_submap_normals: null argument"); return LB_ERR_INVALID_ARG; }
+  if (capacity_points < m->n) { set_error("lb_submap_normals: capacity too small"); return LB_ERR_CAPACITY; }
+  if (m->n == 0) return LB_OK;
+  Ctx& c = m->eng->c;
+  LB_CUDA(cudaSetDevice(c.device));
+  const uint32_t N = (uint32_t)m->n;
+  if (!m->nrm_on) {         // no point has a normal
+    if (mem == LB_MEM_HOST) std::fill(xyz_out, xyz_out + 3 * m->n, std::numeric_limits<float>::quiet_NaN());
+    else {
+      LB_CUDA(cudaMemsetAsync(xyz_out, 0xff, 3 * m->n * sizeof(float), c.stream));
+      LB_CUDA(cudaStreamSynchronize(c.stream));
+    }
+    return LB_OK;
+  }
+  float* d = xyz_out;
+  if (mem == LB_MEM_HOST) { LB_TRY(m->out_xyz.ensure(3 * m->n)); d = m->out_xyz.p; }
+  LB_TRY(m->nn_idx.ensure(m->n));
+  iota_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(m->nn_idx.p, N);
+  sm_gather_xyz_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(m->nrm[m->cur].p, m->nn_idx.p, N, d);
   c.launches += 2;
   if (mem == LB_MEM_HOST) LB_CUDA(cudaMemcpyAsync(xyz_out, d, 3 * m->n * sizeof(float), cudaMemcpyDeviceToHost, c.stream));
   LB_CUDA(cudaStreamSynchronize(c.stream));
@@ -292,6 +367,18 @@ int lb_gicp_set_target_submap(lb_gicp* h, lb_submap* m) {
   const bool reindexed = !(m->indexed_generation == m->generation && e->src->valid);
   LB_TRY(submap_ensure_index(m));
   Cloud& cl = *e->src;
+  if (h->P.recompute_target_covariance == 0 && m->nrm_on && m->n_plain == 0) {
+    // from the stored normals (gicp.hpp:81-82 for a target with normals), as normal_cov_kernel does for an uploaded
+    // cloud; the k-NN cache is left alone
+    if (reindexed || !cl.cov_valid || !m->cov_from_normals || m->nrm_cov_eps != h->P.gicp_epsilon) {
+      LB_TRY(cl.cov.ensure(6 * cl.n));
+      normal_cov_kernel<<<cdiv(cl.n, 256), 256, 0, c.stream>>>(cl.pts.p, m->nrm[m->cur].p, (uint32_t)cl.n, h->P.gicp_epsilon, cl.cov.p);
+      c.launches++;
+      cl.cov_valid = true;
+      m->cov_from_normals = true; m->nrm_cov_eps = h->P.gicp_epsilon;
+    }
+    return submap_adopt(h, m);
+  }
   // covariance cache: everything again when the parameters changed, otherwise only the points inserted since
   if (m->cov_k != k || m->cov_eps != h->P.gicp_epsilon) { m->n_cov = 0; m->cov_k = k; m->cov_eps = h->P.gicp_epsilon; }
   const bool new_cov = m->n_cov < m->n;
@@ -311,12 +398,25 @@ int lb_gicp_set_target_submap(lb_gicp* h, lb_submap* m) {
     c.launches += 2;
     m->n_cov = m->n;
   }
-  if (reindexed || new_cov || !cl.cov_valid) {
+  if (reindexed || new_cov || !cl.cov_valid || m->cov_from_normals) {
     LB_TRY(cl.cov.ensure(6 * cl.n));
     cov_gather_kernel<<<cdiv(6ll * cl.n, 256), 256, 0, c.stream>>>(cl.pts.p, (uint32_t)cl.n, m->cov[m->cur].p, cl.cov.p);
     c.launches++;
     cl.cov_valid = true;
+    m->cov_from_normals = false;
   }
+  return submap_adopt(h, m);
+}
+
+}  // extern "C"
+
+namespace {
+
+// the engine's cloud, its covariances enqueued, becomes h's target
+int submap_adopt(lb_gicp* h, lb_submap* m) {
+  lb_gicp* e = m->eng;
+  Ctx& c = e->c;
+  Cloud& cl = *e->src;
   LB_CUDA(cudaGetLastError());
   if (!cl.ready) LB_CUDA(cudaEventCreateWithFlags(&cl.ready, cudaEventDisableTiming));
   LB_CUDA(cudaEventRecord(cl.ready, c.stream));
@@ -330,6 +430,10 @@ int lb_gicp_set_target_submap(lb_gicp* h, lb_submap* m) {
   LB_CUDA(cudaStreamWaitEvent(h->c.stream, cl.ready, 0));
   return LB_OK;
 }
+
+}  // namespace
+
+extern "C" {
 
 int lb_submap_launch_count(lb_submap* m, uint64_t* n) {
   if (!m || !n) return LB_ERR_INVALID_ARG;

@@ -287,6 +287,8 @@ class B200Odometry {
   }
   lb_gicp_params& params() { return p_; }                       // edit, then applyParams() while the pipeline is idle
   bool applyParams() { return lb_odometry_set_gicp_params(h_, &p_) == LB_OK; }
+  // normals stage (k = 0: off): every filtered scan gets its k-NN normals; idle pipeline, before the first scan
+  bool setNormals(int k, const float* viewpoint = nullptr) { return lb_odometry_set_normals(h_, k, viewpoint) == LB_OK; }
 
   // scan (and filtered_out, if given) must stay valid until next() has returned this ticket
   bool submit(const uint8_t* scan, size_t n_pts, uint32_t point_step, const std::vector<lb_field>& fields,
@@ -322,6 +324,7 @@ class B200Locus {
   }
   lb_locus_params& params() { return p_; }                      // edit, then applyParams() while nothing is in flight
   bool applyParams() { return lb_locus_set_params(h_, &p_) == LB_OK; }
+  // params().front_end: normals and adaptive input voxelization (off by default; shipped values in locus_b200.h)
 
   // scan (and filtered_out, if given) must stay valid until next() has returned this ticket
   bool submit(const uint8_t* scan, size_t n_pts, uint32_t point_step, const std::vector<lb_field>& fields,

@@ -9,6 +9,17 @@ and registration results on the timed scans are checked bit for bit against the 
 (and writes it to --out) with scans/s, the chain's stage times and the card's name, power limit and SM clock.
 
   python tools/bench_locus.py --scans 60 --depth 3 --reps 2 --out /tmp/bench_locus.json
+
+With --front-end the arms are instead, scans on the host:
+  chain_current             lb_locus as above (no normals, k-NN covariances, fixed leaf)
+  chain_shipped             lb_locus in LOCUS's shipped front end: normals k = 20, every covariance from normals,
+                            adaptive input voxelization at 3000 points from a 0.25 leaf
+  seq_shipped               the shipped configuration as blocking calls (computeNormals + an upload with normals,
+                            tools/front_end_oracle.FrontEndChain for the leaf)
+and the line adds the mean leaf and filtered points and how many timed scans were bit-equal between chain_shipped and
+seq_shipped.
+
+  python tools/bench_locus.py --front-end --scans 60 --depth 3 --reps 2
 """
 import argparse
 import ctypes as C
@@ -24,10 +35,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from oracle import locus_oracle as LO  # noqa: E402
+from tools import front_end_oracle as FE  # noqa: E402
 from tools import gen_lidar as G  # noqa: E402
 
 STEP = 32
 LEAF = 0.35
+LEAF_SHIPPED = 0.25       # Locus.cc:39, what the shipped launch sets
 MAP_RES = 0.1
 
 
@@ -96,12 +109,66 @@ def sequential(lb, blobs, d_blobs, prefill, params, device):
     return dt, recs
 
 
-def pipelined(lb, blobs, d_blobs, prefill, params, device, depth):
+def sequential_front_end(lb, blobs, prefill, prefill_n, params):
+    """the shipped front end as blocking calls on the host; returns (seconds, per-scan records)"""
+    import torch
+    P = lb.locus_params(**params)
+    vg = lb.VoxelGridB200(); vg.setFilterFieldName("z"); vg.setFilterLimits(-100.0, 100.0)
+    odo, loc, nrm = lb.GicpB200(), lb.GicpB200(), lb.GicpB200()
+    C.memmove(C.byref(odo._p), C.byref(P.odometry), C.sizeof(P.odometry)); odo._apply()
+    C.memmove(C.byref(loc._p), C.byref(P.localization), C.sizeof(P.localization)); loc._apply()
     m = lb.SubmapB200(0, MAP_RES)
-    m.InsertPoints(prefill)
+    m.InsertPointsWithNormals(prefill, prefill_n)
+    chain = FE.FrontEndChain(P, np.float32(LEAF_SHIPPED))
+    fields = lb.xyzi_fields()
+    recs = []
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    prev = None
+    for b in blobs:
+        leaf = chain.next_leaf
+        vg.setLeafSize(float(leaf))
+        xyz = np.ascontiguousarray(vg.filter(b, STEP, fields)).view(np.float32).reshape(-1, 8)[:, :3].copy()
+        chain.filtered(len(xyz))
+        nrm.setInputSource(xyz)
+        c6 = np.ascontiguousarray(np.hstack([xyz, nrm.computeNormals(0, 20)[:, :3]]))
+        odoT = None
+        if prev is not None:
+            odo.setInputSource(c6, normal_off=12); odo.setInputTarget(prev, normal_off=12)
+            odo.align()
+            odoT = odo.getFinalTransformation()
+        loc.setInputSource(c6, normal_off=12)
+        out = {}
+
+        def localize(Gs):
+            loc.setTargetSubmap(m)
+            out["loc"] = loc.align(Gs)
+            return loc.getFinalTransformation()
+
+        def insert(T):
+            t = loc.transformSource(T, with_normals=True)
+            return m.InsertPointsWithNormals(t[:, :3], t[:, 3:])
+
+        rec = chain.scan(True, odoT, localize, insert, lambda c, half: m.Refresh(c, half))
+        rec["loc_T"] = np.array(out["loc"].final_transformation, np.float32) if "loc" in out else None
+        rec["leaf"] = leaf
+        recs.append(rec)
+        prev = c6
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    m.close()
+    return dt, recs
+
+
+def pipelined(lb, blobs, d_blobs, prefill, params, device, depth, prefill_n=None, leaf=LEAF):
+    m = lb.SubmapB200(0, MAP_RES)
+    if prefill_n is None:
+        m.InsertPoints(prefill)
+    else:
+        m.InsertPointsWithNormals(prefill, prefill_n)
     n = blobs[0].size // STEP
     ch = lb.LocusB200(m, 0, depth=depth, max_points=n, max_point_step=STEP, **params)
-    ch.voxel.setLeafSize(LEAF); ch.voxel.setFilterFieldName("z"); ch.voxel.setFilterLimits(-100.0, 100.0)
+    ch.voxel.setLeafSize(leaf); ch.voxel.setFilterFieldName("z"); ch.voxel.setFilterLimits(-100.0, 100.0)
     fields = lb.api.VoxelGridB200._fields(lb.xyzi_fields())
     res = []
     t0 = time.perf_counter()
@@ -134,6 +201,48 @@ def same(res, recs):
     return bad
 
 
+def front_end(lb, a, blobs, prefill, line):
+    """--front-end: the current chain, the shipped chain and the shipped chain as blocking calls, alternated"""
+    g = lb.GicpB200()
+    g.setInputSource(prefill)
+    prefill_n = g.computeNormals(0, 20)[:, :3].copy()
+    base = dict(translation_threshold_kf=0.6, refresh_every=2)
+    shipped = dict(base, **FE.SHIPPED)
+    line["params"] = dict(base, leaf=LEAF, shipped_front_end=FE.SHIPPED, shipped_initial_leaf=LEAF_SHIPPED,
+                          map_resolution=MAP_RES)
+    arms = ("chain_current", "chain_shipped", "seq_shipped")
+
+    def run(arm):
+        if arm == "chain_current":
+            return pipelined(lb, blobs, None, prefill, base, False, a.depth)
+        if arm == "chain_shipped":
+            return pipelined(lb, blobs, None, prefill, shipped, False, a.depth, prefill_n=prefill_n, leaf=LEAF_SHIPPED)
+        return sequential_front_end(lb, blobs, prefill, prefill_n, shipped)
+
+    for arm in arms:                     # one untimed pass each: modules, allocations
+        run(arm)
+    for rep in range(a.reps):
+        last = {}
+        for arm in arms:
+            out = run(arm)
+            last[arm] = out
+            dt = out[0]
+            entry = dict(scans_per_s=a.scans / dt, ms_per_scan=1e3 * dt / a.scans)
+            if arm.startswith("chain"):
+                res, times = out[1], out[2]
+                entry.update(stage_times=times, filtered_points_mean=float(np.mean([r.n_filtered for r in res])),
+                             leaf_mean=float(np.mean([r.leaf_size for r in res])),
+                             keyframes=sum(r.keyframe for r in res), crops=sum(1 for r in res if r.n_removed))
+            else:
+                entry.update(leaf_mean=float(np.mean([r["leaf"] for r in out[1]])))
+            line["arms"].setdefault(arm, []).append(entry)
+        res, recs = last["chain_shipped"][1], last["seq_shipped"][1]
+        leaves_equal = all(np.float32(r.leaf_size) == e["leaf"] for r, e in zip(res, recs))
+        line["arms"]["chain_shipped"][-1]["bit_equal_scans_vs_seq_shipped"] = (len(res) - same(res, recs)) if leaves_equal else 0
+    for arm in arms:
+        line["best_scans_per_s_" + arm] = max(x["scans_per_s"] for x in line["arms"][arm])
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scans", type=int, default=60)
@@ -143,6 +252,7 @@ def main():
     ap.add_argument("--reps", type=int, default=2)
     ap.add_argument("--seed", type=int, default=5)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--front-end", action="store_true", help="compare the current chain with LOCUS's shipped front end")
     a = ap.parse_args()
     import torch
     import locus_b200 as lb
@@ -151,10 +261,14 @@ def main():
     world = G.world_points(scene, [poses[0], G.pose_matrix([1.0, 0.5, 0.0], [0, 0, 0.3])], a.seed, a.beams, a.az)
     vg = lb.VoxelGridB200(); vg.setLeafSize(0.2)
     prefill = np.ascontiguousarray(vg.filter(G.xyz_blob(world), STEP, lb.xyzi_fields())).view(np.float32).reshape(-1, 8)[:, :3].copy()
-    d_blobs = [torch.from_numpy(b).cuda() for b in blobs]
     params = dict(translation_threshold_kf=0.6, refresh_every=2)
     line = {"scans": a.scans, "raw_points_per_scan": blobs[0].size // STEP, "depth": a.depth, "card": card(),
             "params": dict(params, leaf=LEAF, map_resolution=MAP_RES), "arms": {}}
+    if a.front_end:
+        front_end(lb, a, blobs, prefill, line)
+        emit(line, a.out)
+        return
+    d_blobs = [torch.from_numpy(b).cuda() for b in blobs]
     ref = None
     for arm in ("seq_host", "chain_host", "seq_device", "chain_device"):     # one untimed pass each: modules, allocations
         dev = arm.endswith("device")
@@ -180,12 +294,16 @@ def main():
         s = max(x["scans_per_s"] for x in line["arms"]["seq_" + dev])
         c = max(x["scans_per_s"] for x in line["arms"]["chain_" + dev])
         line["speedup_" + dev] = c / s
+    emit(line, a.out)
+
+
+def emit(line, out):
     line["card_after"] = card()
     txt = json.dumps(line)
     print(txt)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
+    if out:
+        os.makedirs(os.path.dirname(os.path.abspath(out)), exist_ok=True)
+        with open(out, "w") as f:
             f.write(txt + "\n")
 
 
