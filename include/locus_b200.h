@@ -232,6 +232,40 @@ int lb_gicp_fitness(lb_gicp* h, const float* T, double max_range, double* score)
 int lb_gicp_point2plane_information(lb_gicp* h, const void* query, size_t n, size_t q_stride, size_t q_xyz_off,
                                     const void* reference, size_t n_ref, size_t r_stride, size_t r_normal_off,
                                     const int32_t* correspondences, const float* T, int normalize, double* Ap36, int mem);
+/* SURVEY 8f row f1, completed -- the ICP covariance LOCUS's shipped localization computes after every align
+ * (point_cloud_localization/config/parameters.yaml: compute_icp_covariance true, icp_covariance_method 1,
+ * icp_max_covariance 0.01): PointCloudLocalization.cc:325-336 (1-NN of every aligned point) and :398-421, :469-541
+ * (ComputePoint2PlaneICPCovariance).  For the handle's source q (caller order) and its target:
+ *   1. aligned = T q (T NULL = the final transformation), float, as lb_gicp_transform_source;
+ *   2. corr[i] = exact 1-NN of aligned[i] in the target, no distance gate, ties -> lowest index (nearestKSearch(pt, 1));
+ *      or the caller's `correspondences` (n_source int32 target indices, host or device: `mem`) -- then T is not used;
+ *   3. a_i = normalizePCloud(q)[i] (float sums in point order); n_i = the target's normal of corr[i] (the submap's
+ *      stored normal when the target is a submap), rotated by `normal_rotation` (3x3 row-major float, NULL = none) in
+ *      float as transformPointCloudWithNormals rotates normals;
+ *   4. Ap = sum H^T H, H = [a_i x n_i, n_i], rows where a_i or n_i has a NaN skipped (:723-750).  A target point without
+ *      a normal is such a row; a target without normals gives Ap = 0;
+ *   5-9. cov = 0.05^2 Ap^-1, Eigen's LDLT clamp to [1e-12, max_covariance] with the reference's pivot-permuted rebuild,
+ *      the NaN fallbacks and the condition number s0 / s5: locus_b200/csrc/icp_cov.h, which states the Eigen readings.
+ * One stream sequence on the handle's stream (existing transform / 1-NN / normalize / Ap kernels) with one host
+ * synchronisation.  The first search of a target cloud adds one more: the density probe that picks the 1-NN kernel, as in
+ * lb_gicp_nn_target.  A submap target is a new cloud after every change of the map, so in lb_locus the first scan after
+ * a keyframe insert or crop pays two synchronisations here, every other scan one.
+ * Errors: no source LB_ERR_EMPTY_SOURCE; no target LB_ERR_NO_TARGET; T and correspondences both NULL before any align
+ * LB_ERR_NO_ALIGN; a correspondence out of range, or max_covariance not finite or <= 0, LB_ERR_INVALID_ARG.  The
+ * handle's clouds, index, covariances and last align result are never changed.  A submap target must be unchanged
+ * since lb_gicp_set_target_submap (LB_ERR_INVALID_ARG otherwise). */
+#define LB_ICPCOV_CLAMPED 1   /* step 7 clamped a pivot and rebuilt cov */
+#define LB_ICPCOV_D_NAN 2     /* step 6: the LDLT pivots had a NaN -> cov = max I, no condition number */
+#define LB_ICPCOV_COV_NAN 4   /* step 8: cov had a NaN -> max on the diagonal */
+typedef struct lb_icp_covariance {
+  double Ap[36];            /* row-major */
+  double covariance[36];    /* row-major: icp_covariance_ */
+  double condition_number;  /* NaN when step 6 returned early */
+  int flags;                /* LB_ICPCOV_* */
+  size_t n_query, n_used;   /* query points; rows that entered Ap */
+} lb_icp_covariance;
+int lb_gicp_icp_covariance(lb_gicp* h, const float* T, const int32_t* correspondences, int mem, const float* normal_rotation,
+                           double max_covariance, lb_icp_covariance* out);
 /* SURVEY 8f row f2 -- the step right before the path: point_cloud_filter::NormalComputation::filter in its k-NN
  * mode (point_cloud_filter/src/normal_computation.cc:26-59; norm_est_ = pcl::NormalEstimationOMP<PointXYZI, Normal>,
  * normal_computation.h:38; k = normal_search_knn, cfg/NormalComputation.cfg:15).  Per point of the cloud currently set
@@ -542,6 +576,13 @@ typedef struct lb_locus_front_end {
   int points_to_process;      /* points_to_process_in_callback: the filtered point count the leaf aims at (> 0) */
 } lb_locus_front_end;
 
+/* The ICP covariance of the localization (lb_gicp_icp_covariance against the submap after every align); off by default.
+ * Shipped values: enabled = 1, max_covariance = 0.01 (point_cloud_localization/config/parameters.yaml:6,8,10). */
+typedef struct lb_locus_icp_covariance {
+  int enabled;
+  double max_covariance;     /* icp_max_covariance, finite and > 0 */
+} lb_locus_icp_covariance;
+
 typedef struct lb_locus_params {
   lb_gicp_params odometry;               /* k_correspondences, gicp_epsilon and index_cell_size must equal the */
   lb_gicp_params localization;           /* localization's: the shared clouds serve both registrations; so must the
@@ -558,6 +599,7 @@ typedef struct lb_locus_params {
   int prior_map;                         /* b_run_with_gt_point_cloud: localize the first scan against the caller's map */
   double initial_pose[16];               /* row-major; L and the last keyframe before the first scan */
   lb_locus_front_end front_end;          /* normals and adaptive input voxelization (off by default) */
+  lb_locus_icp_covariance icp_covariance;   /* the localization's ICP covariance (off by default) */
 } lb_locus_params;
 
 typedef struct lb_locus_result {
@@ -578,6 +620,17 @@ typedef struct lb_locus_result {
   size_t n_inserted, n_removed;    /* map points added by the insert / removed by the crop of this scan */
   size_t map_size;                 /* after this scan */
   float leaf_size;                 /* the VoxelGrid x leaf this scan was filtered with */
+  /* icp_covariance enabled: the covariance LOCUS publishes in the odometry message's pose.covariance (Locus.cc:510-511),
+   * computed after the localization align and before the keyframe insert, with T = the align's final transformation,
+   * against the submap, the map's normals rotated by the float rotation of P^-1 (P = the align's guess).  Zeros when
+   * the scan was not localized (the first scan without prior_map: PublishPoseNoUpdate, PointCloudLocalization.cc:580-587) */
+  int has_icp_covariance;
+  double icp_covariance[36];
+  double condition_number;         /* the last one computed (Locus.cc:547-548), kept over a scan that took the NaN fallback;
+                                      NaN until the first one is computed (the first scan without prior_map, or a run of
+                                      fallbacks from the start: the reference publishes an uninitialised value there);
+                                      0 when icp_covariance is off */
+  int icp_covariance_flags;        /* LB_ICPCOV_* */
 } lb_locus_result;
 
 /* the reference's shipped values: locus/config/lo_settings.yaml, point_cloud_odometry/config/parameters.yaml,

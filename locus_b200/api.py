@@ -83,12 +83,16 @@ class LocusFrontEnd(C.Structure):
                 ("points_to_process", C.c_int)]
 
 
+class LocusIcpCovariance(C.Structure):
+    _fields_ = [("enabled", C.c_int), ("max_covariance", C.c_double)]
+
+
 class LocusParams(C.Structure):
     _fields_ = [("odometry", GicpParams), ("localization", GicpParams), ("odometry_thresholds", LocusThresholds),
                 ("localization_thresholds", LocusThresholds), ("translation_threshold_kf", C.c_double),
                 ("rotation_threshold_kf", C.c_double), ("add_keyframes", C.c_int), ("refresh_every", C.c_int),
                 ("msw", C.c_int), ("window_half_size", C.c_float), ("prior_map", C.c_int), ("initial_pose", C.c_double * 16),
-                ("front_end", LocusFrontEnd)]
+                ("front_end", LocusFrontEnd), ("icp_covariance", LocusIcpCovariance)]
 
 
 class LocusResult(C.Structure):
@@ -97,7 +101,17 @@ class LocusResult(C.Structure):
                 ("has_localization", C.c_int), ("localization", GicpResult), ("correction_accepted", C.c_int),
                 ("odometry_pose", C.c_double * 16), ("incremental", C.c_double * 16), ("pose", C.c_double * 16),
                 ("keyframe", C.c_int), ("n_inserted", C.c_size_t), ("n_removed", C.c_size_t), ("map_size", C.c_size_t),
-                ("leaf_size", C.c_float)]
+                ("leaf_size", C.c_float), ("has_icp_covariance", C.c_int), ("icp_covariance", C.c_double * 36),
+                ("condition_number", C.c_double), ("icp_covariance_flags", C.c_int)]
+
+
+# lb_icp_covariance.flags
+LB_ICPCOV_CLAMPED, LB_ICPCOV_D_NAN, LB_ICPCOV_COV_NAN = 1, 2, 4
+
+
+class IcpCovariance(C.Structure):
+    _fields_ = [("Ap", C.c_double * 36), ("covariance", C.c_double * 36), ("condition_number", C.c_double),
+                ("flags", C.c_int), ("n_query", C.c_size_t), ("n_used", C.c_size_t)]
 
 
 class VoxelInput(C.Structure):
@@ -128,7 +142,7 @@ SYMBOLS = [
     "lb_gicp_promote_source_to_target", "lb_gicp_reserve", "lb_gicp_prepare_source", "lb_gicp_share_source", "lb_gicp_set_target_cloud",
     "lb_gicp_set_source_cloud",
     "lb_cloud_release", "lb_gicp_align", "lb_gicp_transform_source", "lb_gicp_nn_target",
-    "lb_gicp_fitness", "lb_gicp_point2plane_information", "lb_gicp_compute_normals", "lb_gicp_compute_normals_radius",
+    "lb_gicp_fitness", "lb_gicp_point2plane_information", "lb_gicp_icp_covariance", "lb_gicp_compute_normals", "lb_gicp_compute_normals_radius",
     "lb_gicp_estimate_normals",
     "lb_gicp_statistical_outlier_removal", "lb_gicp_radius_outlier_removal", "lb_gicp_get_covariances", "lb_gicp_cloud_size", "lb_gicp_launch_count",
     "lb_gicp_kernel_time", "lb_gicp_reset_kernel_times",
@@ -204,6 +218,8 @@ def lib():
     L.lb_gicp_nn_target.argtypes = [vp, vp, sz, sz, vp, vp, i32]
     L.lb_gicp_fitness.argtypes = [vp, vp, C.c_double, C.POINTER(C.c_double)]
     L.lb_gicp_point2plane_information.argtypes = [vp, vp, sz, sz, sz, vp, sz, sz, sz, vp, vp, i32, vp, i32]
+    if hasattr(L, "lb_gicp_icp_covariance"):
+        L.lb_gicp_icp_covariance.argtypes = [vp, vp, vp, i32, vp, C.c_double, C.POINTER(IcpCovariance)]
     L.lb_gicp_get_covariances.argtypes = [vp, i32, vp, sz]
     if hasattr(L, "lb_gicp_compute_normals"):
         L.lb_gicp_compute_normals.argtypes = [vp, i32, i32, vp, vp, i32]
@@ -485,6 +501,27 @@ class GicpB200:
         _check(lib().lb_gicp_point2plane_information(self._h, _ptr(q), q.shape[0], 12, 0, _ptr(r), r.shape[0], 12, 0,
                                                      _ptr(co), _ptr(t), int(normalize), _ptr(Ap), LB_MEM_HOST))
         return Ap.reshape(6, 6)
+
+    def icpCovariance(self, T=None, correspondences=None, normal_rotation=None, max_covariance=0.01, device=False):
+        """The ICP covariance after align (PointCloudLocalization.cc:325-336 + ComputePoint2PlaneICPCovariance): the
+        source against the target's normals.  T: 4x4 (None = the final transformation); correspondences: int32 target
+        index per source point (None = the exact 1-NN of T * source), a numpy array or, with device=True, a torch CUDA
+        tensor; normal_rotation: 3x3 applied to the target normals (None = none).  Returns a dict: Ap, covariance (6x6),
+        condition_number (NaN after the D-NaN fallback), flags (LB_ICPCOV_*), n_query, n_used."""
+        t = None if T is None else np.ascontiguousarray(T, dtype=np.float32).reshape(16)
+        r = None if normal_rotation is None else np.ascontiguousarray(normal_rotation, dtype=np.float32).reshape(9)
+        mem, cp = LB_MEM_HOST, None
+        if correspondences is not None:
+            if device:
+                mem, cp = LB_MEM_DEVICE, C.c_void_p(correspondences.data_ptr())
+            else:
+                co = np.ascontiguousarray(correspondences, dtype=np.int32)
+                cp = _ptr(co)
+        out = IcpCovariance()
+        _check(lib().lb_gicp_icp_covariance(self._h, _ptr(t), cp, mem, _ptr(r), float(max_covariance), C.byref(out)))
+        return {"Ap": np.array(out.Ap).reshape(6, 6), "covariance": np.array(out.covariance).reshape(6, 6),
+                "condition_number": out.condition_number, "flags": out.flags, "n_query": out.n_query,
+                "n_used": out.n_used}
 
     def covariances(self, which):
         n = self.cloudSize(which)
@@ -914,7 +951,7 @@ class OdometryB200:
 
 def locus_params(**kw):
     """lb_locus_params with the reference's shipped values; keywords override top-level fields, and `odometry` /
-    `localization` / `*_thresholds` / `front_end` take dicts of their fields"""
+    `localization` / `*_thresholds` / `front_end` / `icp_covariance` take dicts of their fields"""
     p = LocusParams()
     _check(lib().lb_locus_default_params(C.byref(p)))
     for k, v in kw.items():

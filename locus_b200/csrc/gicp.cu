@@ -21,9 +21,13 @@
 
 #include "align_cluster.cuh"
 #include "gicp_kernels.cuh"
+#include "icp_cov.h"
 
 namespace lb {
 const char* last_error();
+// submap.cuh: the normal buffer of a submap whose points a target cloud indexes (nullptr: no point has one);
+// LB_ERR_INVALID_ARG when the map changed since that cloud was built from it
+int submap_target_normals(const lb_submap* m, uint64_t generation, const f4** nrm);
 
 struct Cloud {
   size_t n = 0;
@@ -43,6 +47,9 @@ struct Cloud {
                                // (left there by the accepted round of the occupancy probe)
   uint64_t dense_generation = 0;   // generation for which dense_fraction was measured (lb_gicp_nn_target picks its kernel by it)
   double dense_fraction = 0.0;     // share of the points that sit in cells with more than 32 points
+  // the submap whose points this cloud indexes (its normals live there), and the map generation it was built from
+  const lb_submap* map = nullptr;
+  uint64_t map_generation = 0;
 
   GridView view() const {
     GridView v;
@@ -529,6 +536,7 @@ int upload_cloud(lb_gicp* h, Cloud& cl, int slot, const void* pts, size_t n, siz
   cl.cov_valid = false;
   cl.index_dirty = true;
   cl.generation = ++h->gen_counter;
+  cl.map = nullptr;
   return LB_OK;
 }
 
@@ -1246,21 +1254,11 @@ int lb_gicp_transform_source(lb_gicp* h, const float* T_in, void* out_pts, size_
   return LB_OK;
 }
 
-int lb_gicp_nn_target(lb_gicp* h, const void* xyz, size_t n, size_t stride, int32_t* idx, float* d2, int mem) {
-  if (!h || !xyz || !idx || !d2) { set_error("lb_gicp_nn_target: null argument"); return LB_ERR_INVALID_ARG; }
-  if (!h->tgt->valid) { set_error("lb_gicp_nn_target: no target cloud"); return LB_ERR_NO_TARGET; }
-  if (n == 0) return LB_OK;
-  if ((stride & 3u) || stride < 12) { set_error("lb_gicp_nn_target: bad stride"); return LB_ERR_INVALID_ARG; }
+// Exact 1-NN of N device queries (xyz at the start of each `stride`-byte row) in the prepared target, enqueued on the
+// handle's stream: lb_gicp_nn_target and lb_gicp_icp_covariance.  The kernel is chosen per target by its density over the
+// voxel hash, measured once per target cloud (that measurement synchronises).
+static int nn_search(lb_gicp* h, const uint8_t* dq, uint32_t N, uint32_t stride, int32_t* di, float* dd) {
   Ctx& c = h->c;
-  LB_CUDA(cudaSetDevice(c.device));
-  LB_TRY(prepare_clouds(h, false, false, false));
-  const uint32_t N = (uint32_t)n;
-  const uint8_t* dq = (const uint8_t*)xyz; int32_t* di = idx; float* dd = d2;
-  if (mem == LB_MEM_HOST) {
-    LB_TRY(h->io.ensure(n * stride)); LB_TRY(h->io_idx.ensure(n)); LB_TRY(h->io_d2.ensure(n));
-    LB_CUDA(cudaMemcpyAsync(h->io.p, xyz, n * stride, cudaMemcpyHostToDevice, c.stream));
-    dq = h->io.p; di = h->io_idx.p; dd = h->io_d2.p;
-  }
   if (h->tgt->dense_generation != h->tgt->generation) {      // once per target cloud: how uneven it is over its voxel hash
     Cloud& t = *h->tgt;
     LB_CUDA(cudaMemsetAsync(h->d_debug + 6, 0, sizeof(long long), c.stream));
@@ -1302,6 +1300,25 @@ int lb_gicp_nn_target(lb_gicp* h, const void* xyz, size_t n, size_t stride, int3
     }
     c.launches++;
   }
+  return LB_OK;
+}
+
+int lb_gicp_nn_target(lb_gicp* h, const void* xyz, size_t n, size_t stride, int32_t* idx, float* d2, int mem) {
+  if (!h || !xyz || !idx || !d2) { set_error("lb_gicp_nn_target: null argument"); return LB_ERR_INVALID_ARG; }
+  if (!h->tgt->valid) { set_error("lb_gicp_nn_target: no target cloud"); return LB_ERR_NO_TARGET; }
+  if (n == 0) return LB_OK;
+  if ((stride & 3u) || stride < 12) { set_error("lb_gicp_nn_target: bad stride"); return LB_ERR_INVALID_ARG; }
+  Ctx& c = h->c;
+  LB_CUDA(cudaSetDevice(c.device));
+  LB_TRY(prepare_clouds(h, false, false, false));
+  const uint32_t N = (uint32_t)n;
+  const uint8_t* dq = (const uint8_t*)xyz; int32_t* di = idx; float* dd = d2;
+  if (mem == LB_MEM_HOST) {
+    LB_TRY(h->io.ensure(n * stride)); LB_TRY(h->io_idx.ensure(n)); LB_TRY(h->io_d2.ensure(n));
+    LB_CUDA(cudaMemcpyAsync(h->io.p, xyz, n * stride, cudaMemcpyHostToDevice, c.stream));
+    dq = h->io.p; di = h->io_idx.p; dd = h->io_d2.p;
+  }
+  LB_TRY(nn_search(h, dq, N, (uint32_t)stride, di, dd));
   if (h->timing) {   // profiling aid: mean number of target points a query visits -> h_debug[4], h_debug[5]
     static int nnv2_env = -2;
     if (nnv2_env == -2) { const char* e = getenv("LB_NN"); nnv2_env = !e ? -1 : !strcmp(e, "thread") ? 0 : !strcmp(e, "warp") ? 1 : !strcmp(e, "staged") ? 2 : 3; }
@@ -1388,7 +1405,7 @@ int lb_gicp_point2plane_information(lb_gicp* h, const void* query, size_t n, siz
   ApArgs a;
   a.q = dq; a.n = N; a.q_stride = (uint32_t)q_stride; a.q_xyz_off = (uint32_t)q_xyz_off;
   a.ref = dr; a.n_ref = (uint32_t)n_ref; a.r_stride = (uint32_t)r_stride; a.r_normal_off = (uint32_t)r_normal_off;
-  a.corr = dc; a.norm = nullptr; a.use_R = T ? 1 : 0;
+  a.corr = dc; a.norm = nullptr; a.use_R = T ? 1 : 0; a.use_Rf = 0; a.counters = nullptr;
   for (int i = 0; i < 9; i++) a.R[i] = T ? (double)T[(i / 3) * 4 + (i % 3)] : ((i % 4 == 0) ? 1.0 : 0.0);
   if (normalize) {
     // normalizePCloud's centroid and mean distance, float32 sums in point order like the reference; they stay on the
@@ -1406,6 +1423,82 @@ int lb_gicp_point2plane_information(lb_gicp* h, const void* query, size_t n, siz
   for (int b = 0; b < nb; b++) for (int e = 0; e < 21; e++) up[e] += part[21 * (size_t)b + e];
   int e = 0;
   for (int r = 0; r < 6; r++) for (int cc = r; cc < 6; cc++) { Ap36[r * 6 + cc] = up[e]; Ap36[cc * 6 + r] = up[e]; e++; }
+  return LB_OK;
+}
+
+// SURVEY 8f row f1, completed: PointCloudLocalization.cc:325-336 + ComputePoint2PlaneICPCovariance (:469-541).  The
+// per-point work is the transform, 1-NN, normalize and Ap kernels above, enqueued on the handle's stream into align
+// scratch (src_work: aligned points; corr: indices and distances; M: partials, centroid, counters), then ONE copy-back;
+// the 6x6 algebra runs on the host (icp_cov.h).
+int lb_gicp_icp_covariance(lb_gicp* h, const float* T_in, const int32_t* correspondences, int mem, const float* normal_rotation,
+                           double max_covariance, lb_icp_covariance* out) {
+  if (!h || !out) { set_error("lb_gicp_icp_covariance: null argument"); return LB_ERR_INVALID_ARG; }
+  if (!std::isfinite(max_covariance) || !(max_covariance > 0.0)) {
+    set_error("lb_gicp_icp_covariance: max_covariance must be finite and > 0");
+    return LB_ERR_INVALID_ARG;
+  }
+  if (!h->src->valid) { set_error("lb_gicp_icp_covariance: no source cloud"); return LB_ERR_EMPTY_SOURCE; }
+  if (!h->tgt->valid) { set_error("lb_gicp_icp_covariance: no target cloud"); return LB_ERR_NO_TARGET; }
+  if (!T_in && !correspondences && !h->have_result) { set_error("lb_gicp_icp_covariance: no align() result yet"); return LB_ERR_NO_ALIGN; }
+  Ctx& c = h->c;
+  LB_CUDA(cudaSetDevice(c.device));
+  const Cloud& tg = *h->tgt;
+  const f4* nrm = tg.has_normals ? tg.nrm.p : nullptr;
+  if (tg.map) LB_TRY(submap_target_normals(tg.map, tg.map_generation, &nrm));
+  const uint32_t N = (uint32_t)h->src->n;
+  LB_TRY(h->src_work.ensure(N)); LB_TRY(h->corr.ensure(N));
+  int nb = cdiv(N, 256);
+  if (nb > c.sm_count * 4) nb = c.sm_count * 4;
+  LB_TRY(h->M.ensure((size_t)nb * 21 + 3));
+  float* d_norm = reinterpret_cast<float*>(h->M.p + (size_t)nb * 21);          // 4 floats
+  unsigned* d_cnt = reinterpret_cast<unsigned*>(h->M.p + (size_t)nb * 21 + 2);  // rows used, bad index
+  int32_t* d_corr = reinterpret_cast<int32_t*>(h->corr.p);
+  const int32_t* dc = correspondences;
+  if (!correspondences) {
+    // 1-2: aligned = T q (transformPointCloudWithNormals' float association), exact 1-NN in the target
+    LB_TRY(prepare_clouds(h, false, false, false));
+    Mat34 T; mat16_to_34(T_in ? T_in : h->final_T, T);
+    transform_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(h->src->raw.p, nullptr, N, T, reinterpret_cast<uint8_t*>(h->src_work.p),
+                                                         (uint32_t)sizeof(f4), 0, -1);
+    c.launches++;
+    LB_TRY(nn_search(h, reinterpret_cast<const uint8_t*>(h->src_work.p), N, (uint32_t)sizeof(f4), d_corr,
+                     reinterpret_cast<float*>(h->corr.p) + N));
+    dc = d_corr;
+  } else if (mem == LB_MEM_HOST) {
+    LB_CUDA(cudaMemcpyAsync(d_corr, correspondences, (size_t)N * sizeof(int32_t), cudaMemcpyHostToDevice, c.stream));
+    dc = d_corr;
+  }
+  LB_CUDA(cudaMemsetAsync(d_cnt, 0, 2 * sizeof(unsigned), c.stream));
+  // 3: normalizePCloud(q)'s centroid and mean distance
+  ap_normalize_seq_kernel<<<1, 256, 0, c.stream>>>(reinterpret_cast<const uint8_t*>(h->src->raw.p), N, (uint32_t)sizeof(f4), 0, d_norm);
+  // 4: Ap from the target's own normal buffer, rotated in float
+  ApArgs a;
+  a.q = reinterpret_cast<const uint8_t*>(h->src->raw.p); a.n = N; a.q_stride = (uint32_t)sizeof(f4); a.q_xyz_off = 0;
+  a.ref = reinterpret_cast<const uint8_t*>(nrm); a.n_ref = (uint32_t)tg.n; a.r_stride = (uint32_t)sizeof(f4); a.r_normal_off = 0;
+  a.corr = dc; a.norm = d_norm; a.use_R = 0;
+  for (int i = 0; i < 9; i++) { a.R[i] = 0.0; a.Rf[i] = normal_rotation ? normal_rotation[i] : 0.f; }
+  a.use_Rf = normal_rotation ? 1 : 0;
+  a.counters = d_cnt;
+  ap_accumulate_kernel<<<nb, 256, 0, c.stream>>>(a, h->M.p);
+  c.launches += 2;
+  std::vector<double> part((size_t)nb * 21 + 3);
+  LB_CUDA(cudaMemcpyAsync(part.data(), h->M.p, part.size() * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+  LB_CUDA(cudaStreamSynchronize(c.stream));
+  LB_CUDA(cudaGetLastError());
+  unsigned cnt[2];
+  memcpy(cnt, &part[(size_t)nb * 21 + 2], sizeof(cnt));
+  if (cnt[1]) { set_error("lb_gicp_icp_covariance: a correspondence is outside the target (%zu points)", tg.n); return LB_ERR_INVALID_ARG; }
+  double up[21] = {0};
+  for (int b = 0; b < nb; b++) for (int e = 0; e < 21; e++) up[e] += part[21 * (size_t)b + e];
+  int e = 0;
+  for (int r = 0; r < 6; r++) for (int cc = r; cc < 6; cc++) { out->Ap[r * 6 + cc] = up[e]; out->Ap[cc * 6 + r] = up[e]; e++; }
+  // 5-9 on the host
+  const icpcov::Result res = icpcov::compute(out->Ap, max_covariance);
+  memcpy(out->covariance, res.cov, sizeof(res.cov));
+  out->condition_number = res.condition_number;
+  out->flags = res.flags;
+  out->n_query = N;
+  out->n_used = cnt[0];
   return LB_OK;
 }
 

@@ -2005,6 +2005,11 @@ struct ApArgs {
   const int32_t* corr;
   const float* norm;             // device {cx, cy, cz, dist} of ap_normalize_seq_kernel, or null: no normalisation
   double R[9]; int use_R;        // PointNormal variant rotates the reference normal by R (PointCloudLocalization.cc:715-718)
+  // lb_gicp_icp_covariance: the reference normal rotated by Rf in float first, r = R0 x + (R1 y + R2 z) as
+  // transform_kernel rotates normals (pcl::transformPointCloudWithNormals)
+  float Rf[9]; int use_Rf;
+  // nullable: [0] += rows that entered Ap, [1] |= 1 when a correspondence is out of range
+  unsigned* counters;
 };
 
 __global__ void __launch_bounds__(256)
@@ -2019,14 +2024,22 @@ ap_accumulate_kernel(ApArgs a, double* __restrict__ partials /*[grid][21]*/) {
     factor = (float)a.n / a.norm[3];
     tx = -factor * a.norm[0]; ty = -factor * a.norm[1]; tz = -factor * a.norm[2];
   }
+  unsigned used = 0, bad = 0;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
     const float* p = reinterpret_cast<const float*>(a.q + (size_t)i * a.q_stride + a.q_xyz_off);
     int j = a.corr[i];
-    if (j < 0 || (uint32_t)j >= a.n_ref) continue;
+    if (j < 0 || (uint32_t)j >= a.n_ref) { bad = 1; continue; }
+    if (!a.ref) continue;          // a reference without normals: every row has a NaN normal
     const float* nr = reinterpret_cast<const float*>(a.ref + (size_t)j * a.r_stride + a.r_normal_off);
     double ai[3] = {(double)(factor * p[0] + tx), (double)(factor * p[1] + ty), (double)(factor * p[2] + tz)};
     double ni[3] = {(double)nr[0], (double)nr[1], (double)nr[2]};
+    if (a.use_Rf) {
+      ni[0] = (double)(a.Rf[0] * nr[0] + (a.Rf[1] * nr[1] + a.Rf[2] * nr[2]));
+      ni[1] = (double)(a.Rf[3] * nr[0] + (a.Rf[4] * nr[1] + a.Rf[5] * nr[2]));
+      ni[2] = (double)(a.Rf[6] * nr[0] + (a.Rf[7] * nr[1] + a.Rf[8] * nr[2]));
+    }
     if (isnan(ai[0]) || isnan(ai[1]) || isnan(ai[2]) || isnan(ni[0]) || isnan(ni[1]) || isnan(ni[2])) continue;
+    used++;
     if (a.use_R) {
       double r0 = a.R[0] * ni[0] + a.R[1] * ni[1] + a.R[2] * ni[2];
       double r1 = a.R[3] * ni[0] + a.R[4] * ni[1] + a.R[5] * ni[2];
@@ -2040,6 +2053,14 @@ ap_accumulate_kernel(ApArgs a, double* __restrict__ partials /*[grid][21]*/) {
     for (int r = 0; r < 6; r++)
 #pragma unroll
       for (int c = r; c < 6; c++) acc[e++] += H[r] * H[c];
+  }
+  if (a.counters) {
+    used = __reduce_add_sync(0xffffffffu, used);
+    bad = __reduce_or_sync(0xffffffffu, bad);
+    if ((threadIdx.x & 31) == 0) {
+      if (used) atomicAdd(a.counters, used);
+      if (bad) atomicOr(a.counters + 1, 1u);
+    }
   }
   double tot = block_reduce<21, 8, 0>(acc, red);
   if (threadIdx.x < 21) partials[21 * (size_t)blockIdx.x + threadIdx.x] = tot;

@@ -30,6 +30,7 @@
 #if defined(LB_LOCUS_STUB)       // TEST-ONLY build without CUDA: tests/locus_harness.cpp supplies fake stages
 #include "locus_stub.h"
 #include "front_end_stub.h"
+#include "icp_covariance_stub.h"
 #elif defined(LB_ODOMETRY_STUB)  // TEST-ONLY build without CUDA: tests/odometry_harness.cpp supplies fake stages
 #include "odometry_stub.h"
 #include "front_end_stub.h"
@@ -542,6 +543,7 @@ struct lb_locus {
   bool started = false;            // the first scan has been taken
   lo::Pose O, L, KF;               // odometry estimate, localization estimate, last keyframe
   int counter = 0;                 // keyframes since the last Refresh
+  double condition_number = NAN;   // the last ICP condition number computed (condition_number_, kept over a NaN fallback)
   double t_busy = 0, t_wait = 0;   // core->mu held when updated
   uint64_t n_localized = 0;
   std::thread lthread;
@@ -575,6 +577,21 @@ int locus_localize(lb_locus* c, const lo::Pose& I, size_t n, lb_locus_result& r)
   LB_TRY(lb_gicp_set_target_submap(c->g, c->map));
   LB_TRY(lb_gicp_align(c->g, guess, &r.localization));
   r.has_localization = 1;
+  if (c->P.icp_covariance.enabled) {
+    // PointCloudLocalization.cc:325-336,398-421: the ICP covariance of this align, before the map changes.  The
+    // reference's target is the mapper's neighbours in the frame of P (the align's guess); the submap is in the fixed
+    // frame, so its normals are rotated by P^-1 (unpinned, DESIGN.md 4i)
+    const lo::Pose Pinv = lo::inverse(P);
+    float Rf[9];
+    for (int i = 0; i < 9; i++) Rf[i] = (float)Pinv.R[i];
+    lb_icp_covariance ic;
+    LB_TRY(lb_gicp_icp_covariance(c->g, r.localization.final_transformation, nullptr, LB_MEM_HOST, Rf,
+                                  c->P.icp_covariance.max_covariance, &ic));
+    r.has_icp_covariance = 1;
+    memcpy(r.icp_covariance, ic.covariance, sizeof(r.icp_covariance));
+    r.icp_covariance_flags = ic.flags;
+    if (!(ic.flags & LB_ICPCOV_D_NAN)) c->condition_number = ic.condition_number;
+  }
   const lo::Pose U = lo::delta(P, lo::from_mat(r.localization.final_transformation));   // sensor-frame correction
   const lb_locus_thresholds& th = c->P.localization_thresholds;
   r.correction_accepted = lo::passes(U, th.enabled, th.max_translation, th.max_rotation);
@@ -634,6 +651,7 @@ void locus_scan(lb_locus* c, Entry* e) {
   lo::to_mat(I, r.incremental);
   lo::to_mat(c->L, r.pose);
   lb_submap_size(c->map, &r.map_size);
+  if (c->P.icp_covariance.enabled) r.condition_number = c->condition_number;
 }
 
 void loc_stage(lb_locus* c) {
@@ -683,6 +701,11 @@ int locus_apply_params(lb_locus* c, const lb_locus_params* p) {
   if ((fe.normals_k != 0 && (fe.normals_k < 3 || fe.normals_k > 20)) || (fe.adaptive_voxelization && fe.points_to_process <= 0)) {
     set_error("lb_locus_set_params: front_end needs normals_k = 0 or in [3, 20], and points_to_process > 0 with "
               "adaptive_voxelization");
+    return LB_ERR_INVALID_ARG;
+  }
+  // checked when the covariance is on, so that parameters filled field by field without it keep working
+  if (p->icp_covariance.enabled && (!std::isfinite(p->icp_covariance.max_covariance) || !(p->icp_covariance.max_covariance > 0.0))) {
+    set_error("lb_locus_set_params: icp_covariance.max_covariance must be finite and > 0");
     return LB_ERR_INVALID_ARG;
   }
   LB_TRY(lb_odometry_set_normals(c->core, fe.normals_k, fe.viewpoint));
@@ -740,6 +763,8 @@ int lb_locus_default_params(lb_locus_params* p) {
   p->window_half_size = 20.f;    // box_filter_size
   p->prior_map = 0;              // b_run_with_gt_point_cloud
   for (int i = 0; i < 16; i++) p->initial_pose[i] = (i % 5 == 0) ? 1.0 : 0.0;
+  p->icp_covariance.enabled = 0;               // off: the chain computes what it computed without it
+  p->icp_covariance.max_covariance = 0.01;     // point_cloud_localization/config/parameters.yaml icp_max_covariance
   return LB_OK;
 }
 

@@ -49,6 +49,14 @@ struct lb_submap {
 
 namespace lb {
 int submap_device(const lb_submap* m) { return m->eng->c.device; }   // lb_locus_create checks it against its own
+int submap_target_normals(const lb_submap* m, uint64_t generation, const f4** nrm) {
+  if (m->generation != generation) {
+    set_error("lb_submap: the map changed since lb_gicp_set_target_submap; call it again");
+    return LB_ERR_INVALID_ARG;
+  }
+  *nrm = m->nrm_on ? m->nrm[m->cur].p : nullptr;
+  return LB_OK;
+}
 }  // namespace lb
 
 namespace {
@@ -88,6 +96,7 @@ int submap_ensure_index(lb_submap* m) {
   if (m->n == 0) { set_error("lb_submap: the map is empty"); return LB_ERR_NO_TARGET; }
   LB_TRY(replace_cloud(m->eng, m->eng->src, 0, m->pts[m->cur].p, m->n, sizeof(f4), 0, LB_NO_NORMALS, LB_MEM_DEVICE, "lb_submap"));
   LB_TRY(finish_index(m->eng, *m->eng->src, 0));
+  m->eng->src->map = m; m->eng->src->map_generation = m->generation;
   m->indexed_generation = m->generation;
   return LB_OK;
 }

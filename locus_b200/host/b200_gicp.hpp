@@ -99,6 +99,11 @@ class B200Gicp {
   bool nearestKSearchTarget(const PointF* pts, size_t n, int32_t* idx, float* d2) {
     return lb_gicp_nn_target(h_, pts, n, sizeof(PointF), idx, d2, LB_MEM_HOST) == LB_OK;
   }
+  // the ICP covariance after align (PointCloudLocalization.cc:325-336,398-421): the final transformation, the 1-NN of
+  // every aligned point and the target's normals (rotated by normal_rotation, 3x3 row-major, when given)
+  bool icpCovariance(lb_icp_covariance* out, double max_covariance = 0.01, const float* normal_rotation = nullptr) {
+    return lb_gicp_icp_covariance(h_, nullptr, nullptr, LB_MEM_HOST, normal_rotation, max_covariance, out) == LB_OK;
+  }
   // point_cloud_filter::NormalComputation::filter, k-NN mode (normal_computation.cc:26-59): writes normal_x/y/z of
   // every point of `cloud` (the curvature field is left alone, as the nodelet does).  3 <= k <= 20.
   bool computeNormals(PointF* cloud, size_t n, int k = 20) {

@@ -132,6 +132,30 @@ class B200GeneralizedIterativeClosestPoint : public Registration<PointF, PointF>
     return true;
   }
 
+  // PointCloudLocalization.cc:325-336 + :398-421 in one call after align(): transform the source by the final
+  // transformation, 1-NN of every aligned point in the target, then ComputePoint2PlaneICPCovariance with the target's
+  // normals.  Mat6 is the caller's Eigen::Matrix<double, 6, 6> (icp_covariance_).  *condition_number is left as it was
+  // when the reference returns early (the D-NaN fallback), as condition_number_ is.  false on an error.  The target's
+  // normals reach the GPU only with RecomputeTargetCovariance(false) (what LOCUS ships, recompute_covariance_local_map:
+  // false); otherwise the call is refused rather than answered without normals.
+  template <class Mat6>
+  bool computePoint2PlaneICPCovariance(double max_covariance, Mat6* covariance, double* condition_number) {
+    if (!target_normals_) {
+      PCL_ERROR("[pcl::%s::computePoint2PlaneICPCovariance] the target was uploaded without its normals "
+                "(RecomputeTargetCovariance(true)); set it to false\n", getClassName().c_str());
+      return false;
+    }
+    lb_icp_covariance r;
+    if (lb_gicp_icp_covariance(h_, nullptr, nullptr, LB_MEM_HOST, nullptr, max_covariance, &r) != LB_OK) {
+      PCL_ERROR("[pcl::%s::computePoint2PlaneICPCovariance] %s\n", getClassName().c_str(), lb_last_error_string());
+      return false;
+    }
+    for (int i = 0; i < 6; i++)
+      for (int j = 0; j < 6; j++) (*covariance)(i, j) = r.covariance[6 * i + j];
+    if (!(r.flags & LB_ICPCOV_D_NAN)) *condition_number = r.condition_number;
+    return true;
+  }
+
   const lb_gicp_result& getLastResult() const { return res_; }
   lb_gicp* handle() { return h_; }
 
@@ -177,6 +201,7 @@ class B200GeneralizedIterativeClosestPoint : public Registration<PointF, PointF>
                                               LB_MEM_HOST, nullptr)
                          : lb_gicp_set_source(h_, cloud.points.data(), cloud.size(), sizeof(PointF), offsetof(PointF, x), normal_off,
                                               LB_MEM_HOST);
+    if (s == LB_OK && target) target_normals_ = !recompute;
     if (s != LB_OK) {
       PCL_ERROR("[pcl::%s::%s] %s -- previous input kept\n", getClassName().c_str(), target ? "setInputTarget" : "setInputSource",
                 lb_last_error_string());
@@ -190,6 +215,7 @@ class B200GeneralizedIterativeClosestPoint : public Registration<PointF, PointF>
   lb_gicp_result res_{};
   boost::shared_ptr<B200LazyKdTree<PointF>> lazy_tree_;
   bool source_dirty_ = false, target_dirty_ = false;
+  bool target_normals_ = false;      // the handle's target was uploaded with its normals
 };
 
 }  // namespace pcl

@@ -20,6 +20,13 @@ and the line adds the mean leaf and filtered points and how many timed scans wer
 seq_shipped.
 
   python tools/bench_locus.py --front-end --scans 60 --depth 3 --reps 2
+
+With --icp-covariance the arms are lb_locus in the shipped front end without (shipped_cov_off) and with
+(shipped_cov_on) the localization's ICP covariance (icp_covariance.enabled = 1, max_covariance = 0.01), scans on the host,
+alternated --reps times (default here 3).  Stage L bounds the chain, so its busy time per scan is the cost a user sees;
+the line reports scans/s and stage L busy ms per scan for both arms, and how many timed scans kept bit-equal poses.
+
+  python tools/bench_locus.py --icp-covariance --scans 60 --depth 3 --reps 3
 """
 import argparse
 import ctypes as C
@@ -243,6 +250,37 @@ def front_end(lb, a, blobs, prefill, line):
         line["best_scans_per_s_" + arm] = max(x["scans_per_s"] for x in line["arms"][arm])
 
 
+def icp_covariance(lb, a, blobs, prefill, line):
+    """--icp-covariance: the shipped chain with the ICP covariance off and on, alternated"""
+    g = lb.GicpB200()
+    g.setInputSource(prefill)
+    prefill_n = g.computeNormals(0, 20)[:, :3].copy()
+    base = dict(translation_threshold_kf=0.6, refresh_every=2, **FE.SHIPPED)
+    kw = {"shipped_cov_off": dict(base, icp_covariance=dict(enabled=0, max_covariance=0.01)),
+          "shipped_cov_on": dict(base, icp_covariance=dict(enabled=1, max_covariance=0.01))}
+    line["params"] = dict(base, shipped_initial_leaf=LEAF_SHIPPED, map_resolution=MAP_RES, icp_max_covariance=0.01)
+
+    def run(arm):
+        return pipelined(lb, blobs, None, prefill, kw[arm], False, a.depth, prefill_n=prefill_n, leaf=LEAF_SHIPPED)
+
+    for arm in kw:                       # one untimed pass each: modules, allocations
+        run(arm)
+    for rep in range(a.reps):
+        last = {}
+        for arm in kw:
+            dt, res, times = last[arm] = run(arm)
+            line["arms"].setdefault(arm, []).append(dict(
+                scans_per_s=a.scans / dt, ms_per_scan=1e3 * dt / a.scans,
+                stage_l_busy_ms_per_scan=1e3 * times["localization_busy_s"] / max(times["localized"], 1),
+                stage_times=times, covariances=sum(r.has_icp_covariance for r in res)))
+        off, on = last["shipped_cov_off"][1], last["shipped_cov_on"][1]
+        line["arms"]["shipped_cov_on"][-1]["bit_equal_poses_vs_off"] = sum(
+            np.array_equal(np.asarray(x.pose).view(np.uint64), np.asarray(y.pose).view(np.uint64)) for x, y in zip(off, on))
+    for arm in kw:
+        line["best_scans_per_s_" + arm] = max(x["scans_per_s"] for x in line["arms"][arm])
+        line["median_stage_l_busy_ms_" + arm] = float(np.median([x["stage_l_busy_ms_per_scan"] for x in line["arms"][arm]]))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scans", type=int, default=60)
@@ -253,7 +291,11 @@ def main():
     ap.add_argument("--seed", type=int, default=5)
     ap.add_argument("--out", default=None)
     ap.add_argument("--front-end", action="store_true", help="compare the current chain with LOCUS's shipped front end")
+    ap.add_argument("--icp-covariance", action="store_true",
+                    help="the shipped chain with and without the localization's ICP covariance (--reps defaults to 3)")
     a = ap.parse_args()
+    if a.icp_covariance and "--reps" not in sys.argv:
+        a.reps = 3
     import torch
     import locus_b200 as lb
     assert lb.device_count() > 0, "bench_locus needs a CUDA device"
@@ -266,6 +308,10 @@ def main():
             "params": dict(params, leaf=LEAF, map_resolution=MAP_RES), "arms": {}}
     if a.front_end:
         front_end(lb, a, blobs, prefill, line)
+        emit(line, a.out)
+        return
+    if a.icp_covariance:
+        icp_covariance(lb, a, blobs, prefill, line)
         emit(line, a.out)
         return
     d_blobs = [torch.from_numpy(b).cuda() for b in blobs]

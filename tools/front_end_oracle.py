@@ -19,7 +19,10 @@ tools/bench_locus.py to drive the pre-existing blocking calls with:
       external to the reference, so this arithmetic is unpinned).
 
   FrontEndChain
-      oracle/locus_oracle.py's LocusChain plus the leaf bookkeeping of the callback.
+      oracle/locus_oracle.py's LocusChain plus the leaf bookkeeping of the callback.  With `icp_covariance` enabled it
+      also keeps what stage L hands to lb_gicp_icp_covariance and what it reports: `normal_rotation` (the float32
+      rotation of P^-1 for the scan being localized, P the align's guess, inverted as lo_pose.h inverts it) and
+      `published_condition_number(r)` (the last condition number computed; a D-NaN fallback keeps the previous one).
 """
 import numpy as np
 
@@ -110,6 +113,8 @@ class FrontEndChain(LO.LocusChain):
         super().__init__(params)
         self.leaf = LeafState(leaf0)
         self.next_leaf = np.float32(leaf0)
+        self.normal_rotation = None
+        self.condition_number = float("nan")      # nothing computed yet
 
     def filtered(self, n):
         """the VoxelGrid kept n points with leaf self.next_leaf; returns that leaf and updates it for the next scan"""
@@ -118,3 +123,16 @@ class FrontEndChain(LO.LocusChain):
             if adaptive_leaf(self.leaf, n, self.p.front_end.points_to_process):
                 self.next_leaf = np.float32(self.leaf.leaf)
         return used
+
+    def _localize(self, I, rec, localize, insert, crop):
+        # stage L's normal rotation for this scan: float32 of inverse(P).R, P = update(L, I)
+        P = LO.update(self.L, I)
+        self.normal_rotation = np.array(LO.inverse(P).R, dtype=np.float64).reshape(3, 3).astype(np.float32)
+        return super()._localize(I, rec, localize, insert, crop)
+
+    def published_condition_number(self, result=None):
+        """the condition number lb_locus_result reports after a scan; result: the scan's lb_gicp_icp_covariance output
+        (a dict with condition_number and flags) or None when the scan was not localized"""
+        if result is not None and not (result["flags"] & 2):      # LB_ICPCOV_D_NAN keeps the previous value
+            self.condition_number = result["condition_number"]
+        return self.condition_number
