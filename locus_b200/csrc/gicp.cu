@@ -82,8 +82,8 @@ struct Scratch {
   uint32_t* d_u32 = nullptr; uint32_t* h_u32 = nullptr;
   void release() {
     stage.release(); keys.release(); cell_cnt.release(); worklist.release();
-    sort.ka.release(); sort.kb.release(); sort.va.release(); sort.vb.release(); sort.hist.release();
-    sort.scan.sums.release(); scan.sums.release();
+    sort.ka.release(); sort.kb.release(); sort.va.release(); sort.vb.release(); sort.state.release();
+    scan.sums.release();
     if (d_acc) cudaFree(d_acc);
     if (h_acc) cudaFreeHost(h_acc);
     if (d_u32) cudaFree(d_u32);

@@ -557,8 +557,8 @@ int lb_ndt_destroy(lb_ndt* h) {
   if (h->c.stream) cudaStreamSynchronize(h->c.stream);
   h->src.release(); h->src_spare.release(); h->tgt.release(); h->tgt_spare.release();
   h->keys.release(); h->flag.release(); h->slot_of.release(); h->head_pos.release();
-  h->sort.ka.release(); h->sort.kb.release(); h->sort.va.release(); h->sort.vb.release(); h->sort.hist.release();
-  h->sort.scan.sums.release(); h->scan.sums.release();
+  h->sort.ka.release(); h->sort.kb.release(); h->sort.va.release(); h->sort.vb.release(); h->sort.state.release();
+  h->scan.sums.release();
   h->vox.release(); h->cen.release(); h->leaf_idx.release(); h->hval.release(); h->hkey.release();
   h->io.release(); h->partials.release();
   if (h->d_ctl) cudaFree(h->d_ctl);

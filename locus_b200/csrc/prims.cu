@@ -185,35 +185,60 @@ int exclusive_scan_u32(Ctx& c, ScanWork& w, const uint32_t* in, uint32_t* out, s
 }
 
 // ------------------------------------------------------------------ radix sort
-constexpr int RS_WARPS = 8, RS_ITEMS = 8, RS_TILE = RS_WARPS * 32 * RS_ITEMS;
+constexpr int RS_WARPS = 8, RS_ITEMS = 8;
+static_assert(RS_WARPS * 32 * RS_ITEMS == RS_TILE, "a scatter tile is 256 threads x RS_ITEMS keys");
+static_assert(RS_WARPS * 32 == 256, "one thread per digit");
 
-__global__ void __launch_bounds__(RS_WARPS * 32)
-rs_hist_kernel(const uint32_t* __restrict__ keys, uint32_t n, int shift, uint32_t* __restrict__ block_hist, uint32_t nblocks,
-               const int* __restrict__ key_bits_dev) {
-  __shared__ uint32_t h[256];
-  if (key_bits_dev && shift >= *key_bits_dev) return;     // pass not needed for this key width (known on the device only)
-  h[threadIdx.x] = 0;
-  __syncthreads();
-  uint32_t base = blockIdx.x * RS_TILE;
-#pragma unroll
-  for (int j = 0; j < RS_ITEMS; j++) {
-    uint32_t i = base + j * (RS_WARPS * 32) + threadIdx.x;
-    if (i < n) atomicAdd(&h[(keys[i] >> shift) & 255u], 1u);
+int radix_sort_reserve(Ctx& c, SortWork& w, size_t n) {
+  if (n > 0x7ffffff0ull) { set_error("radix_sort_pairs: n too large"); return LB_ERR_INVALID_ARG; }
+  LB_TRY(w.ka.ensure(n ? n : 1)); LB_TRY(w.kb.ensure(n ? n : 1));
+  LB_TRY(w.va.ensure(n ? n : 1)); LB_TRY(w.vb.ensure(n ? n : 1));
+  const uint32_t tiles = rs_tiles(w.ka.cap);     // sized by the CAPACITY of the key buffers: grows only together with them
+  if (!w.state.p || tiles > w.tiles_cap) {
+    LB_TRY(w.state.ensure(RS_DEV_WORDS + (size_t)RS_PASSES_MAX * tiles * 256));
+    w.tiles_cap = tiles;
+    LB_CUDA(cudaMemsetAsync(w.state.p, 0, sizeof(RsDev), c.stream));      // the zero invariant of a fresh block
   }
-  __syncthreads();
-  block_hist[threadIdx.x * nblocks + blockIdx.x] = h[threadIdx.x];
+  return LB_OK;
 }
 
+// Every pass's digit histogram in one read of the keys (for callers whose key kernel does not fill it); also resets
+// the look-back state of the scatters that follow.
+__global__ void __launch_bounds__(256)
+rs_upsweep_kernel(const uint32_t* __restrict__ keys, uint32_t n, int passes, RsDev* __restrict__ rs, uint32_t* __restrict__ status,
+                  uint32_t tiles) {
+  __shared__ uint32_t sh[RS_PASSES_MAX][256];
+  __shared__ uint32_t scan_sm[256 / 32 + 1];
+  __shared__ bool last;
+  for (int t = threadIdx.x; t < RS_PASSES_MAX * 256; t += 256) (&sh[0][0])[t] = 0;
+  rs_reset_lookback(rs, status, tiles);
+  __syncthreads();
+  for (uint32_t b = blockIdx.x * 256u; b < n; b += gridDim.x * 256u) {      // uniform per CTA: all lanes rank together
+    const uint32_t i = b + threadIdx.x;
+    const bool v = i < n;
+    rs_hist_warp_add(sh, v ? keys[i] : 0u, v, passes);
+  }
+  rs_hist_flush(sh, rs, passes, scan_sm, &last);
+}
+
+// One pass: a tile of RS_TILE keys, taken in ticket order, ranked per warp (__match_any_sync, stable), then its global
+// position per digit = the pass's digit offset + the same digit's count in all earlier tiles, found by decoupled
+// look-back (thread d walks back over digit d's status words).
 __global__ void __launch_bounds__(RS_WARPS * 32)
-rs_scatter_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ vals_in,
-                  uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out, uint32_t n, int shift,
-                  const uint32_t* __restrict__ offsets, uint32_t nblocks, const int* __restrict__ key_bits_dev) {
+rs_onesweep_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ vals_in,
+                   uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out, uint32_t n, int pass,
+                   RsDev* __restrict__ rs, uint32_t* __restrict__ status /*this pass: [tiles][256]*/,
+                   const int* __restrict__ key_bits_dev) {
   __shared__ uint32_t whist[RS_WARPS][256];
-  if (key_bits_dev && shift >= *key_bits_dev) return;
+  __shared__ uint32_t tile_sm;
+  const int shift = 8 * pass;
+  if (key_bits_dev && shift >= *key_bits_dev) return;     // pass not needed for this key width (known on the device only)
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
   for (int i = threadIdx.x; i < RS_WARPS * 256; i += RS_WARPS * 32) (&whist[0][0])[i] = 0;
+  if (threadIdx.x == 0) tile_sm = atomicAdd(&rs->tile_ticket[pass], 1u);
   __syncthreads();
-  const uint32_t warp_base = blockIdx.x * RS_TILE + w * (32 * RS_ITEMS);
+  const uint32_t tile = tile_sm;
+  const uint32_t warp_base = tile * RS_TILE + w * (32 * RS_ITEMS);
   uint32_t key[RS_ITEMS], val[RS_ITEMS], rank[RS_ITEMS];
   const uint32_t lt_mask = (1u << l) - 1u;
 #pragma unroll
@@ -235,115 +260,27 @@ rs_scatter_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __restri
     __syncwarp();
   }
   __syncthreads();
-  // per digit: exclusive scan over the warps of this block, seeded with the global offset
-  {
-    uint32_t d = threadIdx.x;  // RS_WARPS*32 == 256 threads
-    uint32_t run = offsets[d * nblocks + blockIdx.x];
-#pragma unroll
-    for (int ww = 0; ww < RS_WARPS; ww++) {
-      uint32_t cnt = whist[ww][d];
-      whist[ww][d] = run;
-      run += cnt;
-    }
-  }
-  __syncthreads();
-#pragma unroll
-  for (int j = 0; j < RS_ITEMS; j++) {
-    uint32_t i = warp_base + j * 32 + l;
-    if (i < n) {
-      uint32_t d = (key[j] >> shift) & 255u;
-      uint32_t pos = whist[w][d] + rank[j];
-      keys_out[pos] = key[j];
-      vals_out[pos] = val[j];
-    }
-  }
-}
-
-static_assert(RS_WARPS * 32 == 256, "digit scan assumes 256 threads per block");
-
-// Small inputs (<= RS_FUSED_MAX_BLOCKS tiles): no separate scan launches.  The histogram kernel writes block-major
-// counts (coalesced), and every scatter block derives its own 256 offsets from the whole table -- a few coalesced
-// 1 KB reads per tile, L2-resident -- instead of three scan kernels per pass between histogram and scatter.
-constexpr uint32_t RS_FUSED_MAX_BLOCKS = 128;
-
-__global__ void __launch_bounds__(RS_WARPS * 32)
-rs_hist_bm_kernel(const uint32_t* __restrict__ keys, uint32_t n, int shift, uint32_t* __restrict__ block_hist,
-                  const int* __restrict__ key_bits_dev) {
-  __shared__ uint32_t h[256];
-  if (key_bits_dev && shift >= *key_bits_dev) return;
-  h[threadIdx.x] = 0;
-  __syncthreads();
-  uint32_t base = blockIdx.x * RS_TILE;
-#pragma unroll
-  for (int j = 0; j < RS_ITEMS; j++) {
-    uint32_t i = base + j * (RS_WARPS * 32) + threadIdx.x;
-    if (i < n) atomicAdd(&h[(keys[i] >> shift) & 255u], 1u);
-  }
-  __syncthreads();
-  block_hist[blockIdx.x * 256 + threadIdx.x] = h[threadIdx.x];
-}
-
-__global__ void __launch_bounds__(RS_WARPS * 32)
-rs_scatter_fused_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ vals_in,
-                        uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out, uint32_t n, int shift,
-                        const uint32_t* __restrict__ block_hist /*[nblocks][256]*/, uint32_t nblocks,
-                        const int* __restrict__ key_bits_dev) {
-  __shared__ uint32_t whist[RS_WARPS][256];
-  __shared__ uint32_t scan_sm[RS_WARPS + 1];
-  if (key_bits_dev && shift >= *key_bits_dev) return;
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  for (int i = threadIdx.x; i < RS_WARPS * 256; i += RS_WARPS * 32) (&whist[0][0])[i] = 0;
-  // global offset of (digit d = threadIdx.x, this tile): digits below d in all tiles + digit d in the tiles before
-  uint32_t before = 0, total = 0;
   {
     const uint32_t d = threadIdx.x;
-    uint32_t b = 0;
-    for (; b + 4 <= nblocks; b += 4) {
-      uint32_t c0 = block_hist[(b + 0) * 256 + d], c1 = block_hist[(b + 1) * 256 + d];
-      uint32_t c2 = block_hist[(b + 2) * 256 + d], c3 = block_hist[(b + 3) * 256 + d];
-      total += (c0 + c1) + (c2 + c3);
-      before += (b + 0 < blockIdx.x ? c0 : 0u) + (b + 1 < blockIdx.x ? c1 : 0u) + (b + 2 < blockIdx.x ? c2 : 0u) +
-                (b + 3 < blockIdx.x ? c3 : 0u);
-    }
-    for (; b < nblocks; b++) {
-      uint32_t c = block_hist[b * 256 + d];
-      total += c;
-      before += (b < blockIdx.x) ? c : 0u;
-    }
-  }
-  uint32_t all;
-  const uint32_t digit_base = block_excl_scan<RS_WARPS * 32>(total, &all, scan_sm);   // (syncs: whist is zeroed)
-  const uint32_t warp_base = blockIdx.x * RS_TILE + w * (32 * RS_ITEMS);
-  uint32_t key[RS_ITEMS], val[RS_ITEMS], rank[RS_ITEMS];
-  const uint32_t lt_mask = (1u << l) - 1u;
-#pragma unroll
-  for (int j = 0; j < RS_ITEMS; j++) {
-    uint32_t i = warp_base + j * 32 + l;
-    bool valid = i < n;
-    key[j] = valid ? keys_in[i] : 0xffffffffu;
-    val[j] = valid ? (vals_in ? vals_in[i] : i) : 0u;
-    uint32_t d = valid ? ((key[j] >> shift) & 255u) : 256u;
-    uint32_t mask = __match_any_sync(0xffffffffu, d);
-    int leader = __ffs(mask) - 1;
-    uint32_t old = 0;
-    if (l == leader && d < 256u) {
-      old = whist[w][d];
-      whist[w][d] = old + __popc(mask);
-    }
-    old = __shfl_sync(0xffffffffu, old, leader);
-    rank[j] = old + __popc(mask & lt_mask);
-    __syncwarp();
-  }
-  __syncthreads();
-  {
-    uint32_t d = threadIdx.x;
-    uint32_t run = digit_base + before;
+    uint32_t cnt = 0;                     // digit d in this tile; whist becomes each warp's offset within the tile
 #pragma unroll
     for (int ww = 0; ww < RS_WARPS; ww++) {
-      uint32_t cnt = whist[ww][d];
-      whist[ww][d] = run;
-      run += cnt;
+      const uint32_t c = whist[ww][d];
+      whist[ww][d] = cnt;
+      cnt += c;
     }
+    uint32_t* mine = status + (size_t)tile * 256 + d;
+    uint32_t excl = 0;
+    if (tile == 0) {
+      lookback_publish(mine, LB_PREFIX | cnt);
+    } else {
+      lookback_publish(mine, cnt);
+      excl = lookback_prefix(status + d, 256, tile);
+      lookback_publish(mine, LB_PREFIX | (excl + cnt));
+    }
+    const uint32_t off = rs->base[pass][d] + excl;
+#pragma unroll
+    for (int ww = 0; ww < RS_WARPS; ww++) whist[ww][d] += off;
   }
   __syncthreads();
 #pragma unroll
@@ -360,37 +297,26 @@ rs_scatter_fused_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __
 
 // key_bits_dev != nullptr: the key width is only known on the device (lb_voxel_filter: it follows from the bounding box
 // of the call's own input).  `key_bits` is then the host's upper bound: that many bits' worth of passes are LAUNCHED,
-// and the kernels of a pass whose digit lies beyond *key_bits_dev return at once -- the executed passes are a prefix, so
-// the result sits in buffer A (w.ka / w.va) after an odd number of executed passes and in B after an even number (> 0).
+// and a pass whose digit lies beyond *key_bits_dev returns at once -- the executed passes are a prefix, so the result
+// sits in buffer A (w.ka / w.va) after an odd number of executed passes and in B after an even number (> 0).
 static int radix_sort_impl(Ctx& c, SortWork& w, const uint32_t* keys_in, const uint32_t* vals_in, size_t n, int key_bits,
-                           const int* key_bits_dev, uint32_t** keys_out, uint32_t** vals_out) {
-  if (n > 0xfffffff0ull) { set_error("radix_sort_pairs: n too large"); return LB_ERR_INVALID_ARG; }
-  LB_TRY(w.ka.ensure(n ? n : 1)); LB_TRY(w.kb.ensure(n ? n : 1));
-  LB_TRY(w.va.ensure(n ? n : 1)); LB_TRY(w.vb.ensure(n ? n : 1));
-  uint32_t nblocks = (uint32_t)((n + RS_TILE - 1) / RS_TILE);
-  if (nblocks == 0) nblocks = 1;
-  {   // sized by the CAPACITY of the key buffers, so that it only ever grows together with them
-    const size_t nb_cap = (w.ka.cap + RS_TILE - 1) / RS_TILE;
-    LB_TRY(w.hist.ensure((size_t)256 * (nb_cap > nblocks ? nb_cap : nblocks)));
-  }
+                           const int* key_bits_dev, bool histogram, uint32_t** keys_out, uint32_t** vals_out) {
+  LB_TRY(radix_sort_reserve(c, w, n));
+  const uint32_t tiles = rs_tiles(n);
   int passes = (key_bits + 7) / 8;
   if (passes < 1) passes = 1;
+  if (passes > RS_PASSES_MAX) passes = RS_PASSES_MAX;
+  if (histogram) {
+    const uint32_t grid = tiles < (uint32_t)(2 * c.sm_count) ? tiles : (uint32_t)(2 * c.sm_count);
+    rs_upsweep_kernel<<<grid, 256, 0, c.stream>>>(keys_in, (uint32_t)n, passes, w.dev(), w.status(), tiles);
+    c.launches++;
+  }
   const uint32_t* kin = keys_in; const uint32_t* vin = vals_in;
   uint32_t* kout = w.ka.p; uint32_t* vout = w.va.p;
-  const bool fused = nblocks <= RS_FUSED_MAX_BLOCKS;
   for (int p = 0; p < passes; p++) {
-    int shift = 8 * p;
-    if (fused) {
-      rs_hist_bm_kernel<<<nblocks, RS_WARPS * 32, 0, c.stream>>>(kin, (uint32_t)n, shift, w.hist.p, key_bits_dev);
-      rs_scatter_fused_kernel<<<nblocks, RS_WARPS * 32, 0, c.stream>>>(kin, vin, kout, vout, (uint32_t)n, shift, w.hist.p, nblocks, key_bits_dev);
-      c.launches += 2;
-    } else {
-      rs_hist_kernel<<<nblocks, RS_WARPS * 32, 0, c.stream>>>(kin, (uint32_t)n, shift, w.hist.p, nblocks, key_bits_dev);
-      c.launches++;
-      LB_TRY(exclusive_scan_u32(c, w.scan, w.hist.p, w.hist.p, (size_t)256 * nblocks, nullptr));
-      rs_scatter_kernel<<<nblocks, RS_WARPS * 32, 0, c.stream>>>(kin, vin, kout, vout, (uint32_t)n, shift, w.hist.p, nblocks, key_bits_dev);
-      c.launches++;
-    }
+    rs_onesweep_kernel<<<tiles, RS_WARPS * 32, 0, c.stream>>>(kin, vin, kout, vout, (uint32_t)n, p, w.dev(),
+                                                               w.status() + (size_t)p * tiles * 256, key_bits_dev);
+    c.launches++;
     kin = kout; vin = vout;
     if (kout == w.ka.p) { kout = w.kb.p; vout = w.vb.p; } else { kout = w.ka.p; vout = w.va.p; }
   }
@@ -402,11 +328,11 @@ static int radix_sort_impl(Ctx& c, SortWork& w, const uint32_t* keys_in, const u
 
 int radix_sort_pairs(Ctx& c, SortWork& w, const uint32_t* keys_in, const uint32_t* vals_in, size_t n, int key_bits,
                      uint32_t** keys_out, uint32_t** vals_out) {
-  return radix_sort_impl(c, w, keys_in, vals_in, n, key_bits, nullptr, keys_out, vals_out);
+  return radix_sort_impl(c, w, keys_in, vals_in, n, key_bits, nullptr, true, keys_out, vals_out);
 }
 
 int radix_sort_pairs_devbits(Ctx& c, SortWork& w, const uint32_t* keys_in, size_t n, int max_key_bits, const int* key_bits_dev) {
-  return radix_sort_impl(c, w, keys_in, nullptr, n, max_key_bits, key_bits_dev, nullptr, nullptr);
+  return radix_sort_impl(c, w, keys_in, nullptr, n, max_key_bits, key_bits_dev, false, nullptr, nullptr);
 }
 
 }  // namespace lb

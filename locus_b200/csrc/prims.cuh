@@ -157,19 +157,107 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* total,
 struct ScanWork { DBuf<uint32_t> sums; };
 int exclusive_scan_u32(Ctx& c, ScanWork& w, const uint32_t* in, uint32_t* out, size_t n, uint32_t* total_dev);
 
+// ------------------------------------------------------------------ decoupled look-back
+// A tile status word: LB_NOT_READY, or a count of the tile alone (bit 31 clear) or the inclusive prefix over the tile
+// and every tile before it (bit 31 set).  Counts stay below 2^31 - 1, so no published word equals LB_NOT_READY.
+constexpr uint32_t LB_NOT_READY = 0xffffffffu, LB_PREFIX = 0x80000000u;
+
+__device__ __forceinline__ void lookback_publish(uint32_t* w, uint32_t v) { *reinterpret_cast<volatile uint32_t*>(w) = v; }
+
+// Exclusive prefix of tile `tile` from the status words of the tiles before it (word of tile j at status[j * stride]).
+// Tile ids come from an atomic ticket taken at CTA start, so every tile waited on has started and publishes its own
+// count without waiting on anyone: the walk always ends.
+__device__ __forceinline__ uint32_t lookback_prefix(const uint32_t* status, size_t stride, uint32_t tile) {
+  uint32_t excl = 0;
+  for (int64_t j = (int64_t)tile - 1; j >= 0;) {
+    const uint32_t s = *reinterpret_cast<const volatile uint32_t*>(status + (size_t)j * stride);
+    if (s == LB_NOT_READY) continue;
+    excl += s & ~LB_PREFIX;
+    if (s & LB_PREFIX) break;
+    j--;
+  }
+  return excl;
+}
+
 // ------------------------------------------------------------------ sort
-// Stable LSD radix sort of (key, val) pairs on the low `key_bits` bits.
+// Stable LSD radix sort of (key, val) pairs on the low `key_bits` bits, 8-bit digits, one sweep per pass: one read of
+// the keys fills every pass's digit histogram, then each pass is ONE scatter kernel whose tiles find their global digit
+// offsets by decoupled look-back over per-tile, per-digit status words.
 // vals_in == nullptr means val = element index.  Result ends in *keys_out/*vals_out
 // (pointers into the ping-pong buffers a/b).
-struct SortWork {
-  DBuf<uint32_t> ka, kb, va, vb, hist;
-  ScanWork scan;
+constexpr int RS_PASSES_MAX = 4;
+constexpr int RS_TILE = 2048;              // keys per scatter tile (256 threads x 8)
+
+// Device state of one SortWork, followed in memory by the tile status words (RS_PASSES_MAX x tiles x 256).
+// Invariant between sorts: `acc` and `hist_ticket` are zero.  The histogram's last CTA turns `acc` into `base` and
+// zeroes it; the kernel that fills the histogram also resets the status words and `tile_ticket` of the passes after it.
+struct RsDev {
+  uint32_t acc[RS_PASSES_MAX][256];        // digit counts of every pass (atomics of the histogram CTAs)
+  uint32_t base[RS_PASSES_MAX][256];       // exclusive digit offsets of every pass (read by the scatters)
+  uint32_t hist_ticket;                    // last-CTA detection of the histogram
+  uint32_t tile_ticket[RS_PASSES_MAX];     // tile ids of the scatter passes
+  uint32_t pad[3];
 };
+constexpr size_t RS_DEV_WORDS = sizeof(RsDev) / 4;
+
+struct SortWork {
+  DBuf<uint32_t> ka, kb, va, vb;
+  DBuf<uint32_t> state;                    // RsDev + status words
+  uint32_t tiles_cap = 0;                  // tiles the status words are sized for
+  RsDev* dev() const { return reinterpret_cast<RsDev*>(state.p); }
+  uint32_t* status() const { return state.p + RS_DEV_WORDS; }
+};
+static inline uint32_t rs_tiles(size_t n) { uint32_t t = (uint32_t)((n + RS_TILE - 1) / RS_TILE); return t ? t : 1; }
+
+// Buffers for n keys (grown, never shrunk; a fresh state block is zeroed once, on the stream).
+int radix_sort_reserve(Ctx& c, SortWork& w, size_t n);
+
+// ---- the histogram, for kernels that already touch every key (256-thread CTAs)
+// sh: __shared__ uint32_t[RS_PASSES_MAX][256], zeroed and synchronised by the caller.  All 32 lanes call it.
+__device__ __forceinline__ void rs_hist_warp_add(uint32_t (*sh)[256], uint32_t key, bool valid, int passes) {
+#pragma unroll
+  for (int p = 0; p < RS_PASSES_MAX; p++) {
+    if (p >= passes) break;
+    const uint32_t d = valid ? ((key >> (8 * p)) & 255u) : 256u;
+    const uint32_t m = __match_any_sync(0xffffffffu, d);
+    if (d < 256u && (threadIdx.x & 31) == __ffs(m) - 1) atomicAdd(&sh[p][d], (uint32_t)__popc(m));
+  }
+}
+// After the CTA's keys are in `sh`: one global atomic per non-zero digit, then the last CTA of the grid turns the
+// totals into exclusive digit offsets and restores the zero invariant.  Call with the whole CTA (256 threads).
+__device__ __forceinline__ void rs_hist_flush(uint32_t (*sh)[256], RsDev* rs, int passes, uint32_t* scan_sm /*9*/, bool* last_sm) {
+  __syncthreads();
+  const uint32_t d = threadIdx.x;
+  for (int p = 0; p < passes; p++)
+    if (sh[p][d]) atomicAdd(&rs->acc[p][d], sh[p][d]);
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) *last_sm = atomicAdd(&rs->hist_ticket, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!*last_sm) return;
+  __threadfence();
+  for (int p = 0; p < passes; p++) {
+    const uint32_t v = atomicExch(&rs->acc[p][d], 0u);
+    uint32_t tot;
+    rs->base[p][d] = block_excl_scan<256>(v, &tot, scan_sm);
+  }
+  if (threadIdx.x == 0) rs->hist_ticket = 0;
+}
+// Status words and tile tickets of the scatters that follow (grid-stride; any grid that runs before them).
+__device__ __forceinline__ void rs_reset_lookback(RsDev* rs, uint32_t* status, uint32_t tiles) {
+  const size_t words = (size_t)RS_PASSES_MAX * tiles * 256;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < words; i += (size_t)gridDim.x * blockDim.x)
+    status[i] = LB_NOT_READY;
+  if (blockIdx.x == 0 && threadIdx.x < RS_PASSES_MAX) rs->tile_ticket[threadIdx.x] = 0;
+}
+
 int radix_sort_pairs(Ctx& c, SortWork& w, const uint32_t* keys_in, const uint32_t* vals_in, size_t n, int key_bits,
                      uint32_t** keys_out, uint32_t** vals_out);
-// Same sort (val = element index) when the key width is only known on the device: passes for max_key_bits are launched,
-// those beyond *key_bits_dev return at once.  Result: buffers w.ka / w.va after an odd number of executed passes
-// ((*key_bits_dev + 7) / 8), w.kb / w.vb after an even number; consumers pick on the device.
+// The scatter passes only (val = element index), for a caller whose own key kernel filled the histogram
+// (rs_hist_warp_add / rs_hist_flush) and reset the look-back (rs_reset_lookback) after radix_sort_reserve.  The key
+// width is only known on the device: passes for max_key_bits are launched, those beyond *key_bits_dev return at once.
+// Result: buffers w.ka / w.va after an odd number of executed passes ((*key_bits_dev + 7) / 8), w.kb / w.vb after an
+// even number; consumers pick on the device.
 int radix_sort_pairs_devbits(Ctx& c, SortWork& w, const uint32_t* keys_in, size_t n, int max_key_bits, const int* key_bits_dev);
 
 }  // namespace lb

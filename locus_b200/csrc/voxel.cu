@@ -6,14 +6,17 @@
 //
 // One call = one stream-ordered chain of kernels with NO host round trip in between: everything a later kernel needs
 // from an earlier one (bounding box -> min_b / div_b / key width, voxel count) stays in a small device-resident state
-// block; the host synchronises once, at the end, to learn the voxel count and the status.
+// block; the host synchronises once, at the end, to learn the voxel count and the status.  3 + (sort passes) kernels:
 //   vg_bbox_kernel     finite + filter-limit + body-box predicate, min/max reduce (two 16-byte loads per 32-byte
 //                      record); the last CTA derives min_b, div_b, the overflow guard and the key width
 //   vg_keys_kernel     int32 PCL leaf index per point (bit-exact float32 math) + a packed float4 record of the four
-//                      averaged fields, so that no later kernel touches the raw cloud's strided layout again
-//   radix sort         stable LSD sort of (leaf index, point#); passes beyond the key width return at once
-//   vg_tile_heads_kernel + vg_segstart_kernel    voxel segments (per-tile head counts, then prefix + local scan)
-//   vg_centroid4_kernel   a warp owns 32 consecutive voxels: float32 sum in ascending point order, / count
+//                      averaged fields, so that no later kernel touches the raw cloud's strided layout again; also
+//                      every sort pass's digit histogram, and the reset of the look-back state of the kernels after it
+//   radix sort         one scatter kernel per pass of the stable LSD sort of (leaf index, point#); passes beyond the
+//                      key width return at once
+//   vg_segment_kernel  tiles of sorted positions: voxel heads, min_points_per_voxel, output slots by decoupled
+//                      look-back, and one lane per voxel summing it in float32 in ascending point order, / count; the
+//                      last tile writes the call's state into pinned host memory (no copy in the chain)
 // Algorithmic bytes: N_in*point_step + N_out*point_step (SURVEY 8d).
 #include <float.h>
 #include <math.h>
@@ -37,17 +40,17 @@ struct VoxelFieldsDev {
   uint32_t ff_off[VG_MAX_FIELDS];
 };
 
-// device-resident state of one lb_voxel_filter call (written by the kernels, read back once at the end)
+// device-resident state of one lb_voxel_filter call (written by the kernels; vg_segment_kernel hands it to the host)
 struct VoxState {
   BBoxAcc acc;                 // bounding box of the surviving points; reset by the CTA that consumes it
   unsigned ticket;             // last-CTA detection of vg_bbox_kernel
+  unsigned seg_ticket;         // tile ids of vg_segment_kernel; reset by vg_bbox_kernel
   int status;                  // LB_OK or LB_ERR_VOXEL_OVERFLOW
   int min_b[3], div_b[3];
   uint32_t sentinel;           // number of cells of the grid = key of a dropped point (sorts last)
   int key_bits;                // width of the sort key; 0: nothing to do (empty input / overflow)
   uint32_t count;              // surviving points
-  uint32_t n_seg;              // occupied voxels
-  uint32_t n_final;            // output points (after min_points_per_voxel)
+  uint32_t n_final;            // output points (occupied voxels after min_points_per_voxel)
 };
 
 struct VoxLimits {
@@ -199,18 +202,16 @@ vg_bbox_kernel(const __grid_constant__ VoxInputs in, uint32_t n, uint32_t stride
     }
   }
   st->status = status; st->sentinel = sentinel; st->key_bits = key_bits; st->count = count;
-  st->n_seg = 0; st->n_final = 0;
+  st->n_final = 0;
   bbox_reset(&st->acc);            // consumed: clean for the next call
   st->ticket = 0;
+  st->seg_ticket = 0;
 }
 
-__global__ void __launch_bounds__(256)
-vg_keys_kernel(const __grid_constant__ VoxInputs in, uint32_t n, uint32_t stride, uint32_t xyz_off, VoxLimits lim, BodyBox body,
-               float inv0, float inv1, float inv2, int vec32, VoxelFieldsDev F, const VoxState* __restrict__ st,
-               uint32_t* __restrict__ keys, float4* __restrict__ rec /*nullable: only for 4 averaged fields*/) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int key_bits = st->key_bits;
-  if (key_bits == 0 || i >= n) return;              // empty input or overflow: nothing is sorted
+// the sort key (PCL leaf index, or the sentinel for a dropped point) and the averaged record of point i
+__device__ __forceinline__ uint32_t vg_point_key(const VoxInputs& in, uint32_t i, uint32_t stride, uint32_t xyz_off, const VoxLimits& lim,
+                                                 const BodyBox& body, float inv0, float inv1, float inv2, int vec32,
+                                                 const VoxelFieldsDev& F, const VoxState* __restrict__ st, float4* __restrict__ rec) {
   const uint32_t sentinel = st->sentinel;
   const int min_b0 = st->min_b[0], min_b1 = st->min_b[1], min_b2 = st->min_b[2];
   const int mul1 = st->div_b[0], mul2 = st->div_b[0] * st->div_b[1];
@@ -256,232 +257,266 @@ vg_keys_kernel(const __grid_constant__ VoxInputs in, uint32_t n, uint32_t stride
     const int idx = ijk0 + ijk1 * mul1 + ijk2 * mul2;
     key = ((uint32_t)idx < sentinel) ? (uint32_t)idx : sentinel;
   }
-  keys[i] = key;
   if (rec) rec[i] = r4;
+  return key;
+}
+
+constexpr int VG_KEYS_ITEMS = 4;     // points per thread of vg_keys_kernel: 1024 per CTA, one histogram flush each
+
+// Keys + records, and the digit histogram of every sort pass the key width needs (one atomic per non-zero digit and
+// CTA, the last CTA turns them into digit offsets).  Also resets the look-back state of the sort's scatters and of
+// vg_segment_kernel: every kernel after this one starts from clean status words.
+__global__ void __launch_bounds__(256)
+vg_keys_kernel(const __grid_constant__ VoxInputs in, uint32_t n, uint32_t stride, uint32_t xyz_off, VoxLimits lim, BodyBox body,
+               float inv0, float inv1, float inv2, int vec32, VoxelFieldsDev F, const VoxState* __restrict__ st,
+               uint32_t* __restrict__ keys, float4* __restrict__ rec /*nullable: only for 4 averaged fields*/,
+               RsDev* __restrict__ rs, uint32_t* __restrict__ rs_status, uint32_t rs_tiles,
+               uint32_t* __restrict__ seg_status, uint32_t seg_tiles) {
+  __shared__ uint32_t sh[RS_PASSES_MAX][256];
+  __shared__ uint32_t scan_sm[256 / 32 + 1];
+  __shared__ bool last;
+  const int key_bits = st->key_bits;
+  if (key_bits == 0) return;              // empty input or overflow: nothing is sorted
+  const int passes = (key_bits + 7) >> 3;
+  for (int t = threadIdx.x; t < RS_PASSES_MAX * 256; t += 256) (&sh[0][0])[t] = 0;
+  rs_reset_lookback(rs, rs_status, rs_tiles);
+  for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < seg_tiles; t += gridDim.x * blockDim.x) seg_status[t] = LB_NOT_READY;
+  __syncthreads();
+#pragma unroll 1
+  for (int u = 0; u < VG_KEYS_ITEMS; u++) {
+    const uint32_t i = blockIdx.x * (256u * VG_KEYS_ITEMS) + u * 256u + threadIdx.x;
+    uint32_t key = 0;
+    if (i < n) {
+      key = vg_point_key(in, i, stride, xyz_off, lim, body, inv0, inv1, inv2, vec32, F, st, rec);
+      keys[i] = key;
+    }
+    rs_hist_warp_add(sh, key, i < n, passes);
+  }
+  rs_hist_flush(sh, rs, passes, scan_sm, &last);
 }
 
 // which ping-pong buffer holds the sorted pairs: A after an odd number of executed passes, B after an even number
 __device__ __forceinline__ bool vg_sorted_in_a(int key_bits) { return (((key_bits + 7) >> 3) & 1) != 0; }
 
-constexpr int VG_TILE = 2048;      // sorted positions per CTA of the two segment kernels (256 threads x 8)
-
-__device__ __forceinline__ uint32_t vg_head_flags8(const uint32_t* __restrict__ keys, uint32_t base, uint32_t n, uint32_t sentinel,
-                                                   uint32_t* cnt) {
-  // 8 consecutive sorted positions per thread; bit j: position base + j starts a voxel
-  uint32_t bits = 0, c = 0;
-  uint32_t prev = (base > 0 && base <= n) ? keys[base - 1] : 0xffffffffu;
+// lookback_prefix by a whole warp over consecutive status words, 32 tiles per step; every lane returns the prefix.
+__device__ __forceinline__ uint32_t lookback_prefix_warp(const uint32_t* status, uint32_t tile) {
+  const int lane = threadIdx.x & 31;
+  uint32_t excl = 0;
+  for (int64_t top = (int64_t)tile - 1;; top -= 32) {         // lane 0 reads the nearest earlier tile
+    const int64_t j = top - lane;
+    const volatile uint32_t* w = status + (j >= 0 ? j : 0);
+    uint32_t s = (j >= 0) ? *w : LB_PREFIX;                    // before tile 0: a prefix of 0
+    while (__any_sync(0xffffffffu, s == LB_NOT_READY))
+      if (s == LB_NOT_READY) s = *w;
+    const uint32_t pm = __ballot_sync(0xffffffffu, (s & LB_PREFIX) != 0);
+    const int stop = pm ? __ffs(pm) - 1 : 31;                  // the nearest prefix ends the walk
+    uint32_t v = (lane <= stop) ? (s & ~LB_PREFIX) : 0u;
 #pragma unroll
-  for (int j = 0; j < 8; j++) {
-    const uint32_t i = base + j;
-    if (i < n) {
-      const uint32_t k = keys[i];
-      if (k < sentinel && (i == 0 || k != prev)) { bits |= 1u << j; c++; }
-      prev = k;
-    }
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    excl += v;
+    if (pm) return excl;
   }
-  *cnt = c;
-  return bits;
 }
 
+constexpr int VG_SEG_TILE = 1024;    // sorted positions per CTA of vg_segment_kernel (256 threads x 4)
+
+// One tile of sorted positions, taken in ticket order:
+//   1. the positions where the key changes (voxel heads, and the start of the dropped points' sentinel run)
+//   2. the end of the voxel that crosses the tile end: one warp reads on, 32 keys per step
+//   3. FOUR: the packed float4 records of the tile and of that crossing tail (up to another tile's worth) staged in
+//      shared memory (coalesced point numbers, 16-byte gathers, all in flight at once); and per voxel that STARTS in the tile: its end (the next head, or the crossing tail's end) and whether it holds
+//      min_points_per_voxel points
+//   4. output slots: the kept voxels of the tile in order, after those of every earlier tile (decoupled look-back)
+//   5. one lane per voxel: float32 sum of its records in ascending input order (the order the stable sort produced;
+//      it defines the rounding: PCL's centroid += point, then /= float(n)), records past the tile end read from
+//      global memory; other layouts read the caller's bytes through the sorted point numbers
+// The last tile knows the voxel count: it writes the call's whole state into pinned host memory.
+template <bool FOUR>
 __global__ void __launch_bounds__(256)
-vg_tile_heads_kernel(const uint32_t* __restrict__ ka, const uint32_t* __restrict__ kb, const VoxState* __restrict__ st, uint32_t n,
-                     uint32_t* __restrict__ tile_cnt) {
-  __shared__ uint32_t sm[256 / 32 + 1];
+vg_segment_kernel(const __grid_constant__ VoxInputs in, uint32_t stride, const uint32_t* __restrict__ ka, const uint32_t* __restrict__ kb,
+                  const uint32_t* __restrict__ va, const uint32_t* __restrict__ vb, const float4* __restrict__ rec,
+                  VoxState* __restrict__ st, VoxState* __restrict__ h_st, uint32_t* __restrict__ seg_status, uint32_t n,
+                  int min_points, VoxelFieldsDev F, uint32_t capacity, int vec32, uint8_t* __restrict__ out,
+                  int32_t* __restrict__ out_voxel_idx) {
+  __shared__ uint32_t bnd[VG_SEG_TILE];      // tile positions where the key changes, ascending
+  __shared__ uint32_t endp[VG_SEG_TILE];     // end of the voxel starting at bnd[h]; 0: not an output voxel
+  __shared__ uint32_t slot[VG_SEG_TILE];     // its rank among the tile's output voxels
+  __shared__ float4 recs[FOUR ? 2 * VG_SEG_TILE : 1];   // sorted positions t0 .. staged end
+  __shared__ uint32_t scan_sm[256 / 32 + 1];
+  __shared__ uint32_t tile_sm, pre_sm, tail_sm;
   const int key_bits = st->key_bits;
-  if (key_bits == 0) { if (threadIdx.x == 0) tile_cnt[blockIdx.x] = 0; return; }
-  const uint32_t* keys = vg_sorted_in_a(key_bits) ? ka : kb;
-  uint32_t c;
-  vg_head_flags8(keys, blockIdx.x * VG_TILE + threadIdx.x * 8, n, st->sentinel, &c);
-  uint32_t tot;
-  block_excl_scan<256>(c, &tot, sm);
-  if (threadIdx.x == 0) tile_cnt[blockIdx.x] = tot;
-}
-
-// seg_start[s] = sorted position where voxel s begins; the last CTA publishes the voxel count
-__global__ void __launch_bounds__(256)
-vg_segstart_kernel(const uint32_t* __restrict__ ka, const uint32_t* __restrict__ kb, VoxState* __restrict__ st, uint32_t n,
-                   const uint32_t* __restrict__ tile_cnt, uint32_t* __restrict__ seg_start) {
-  __shared__ uint32_t sm[256 / 32 + 1];
-  __shared__ uint32_t pre_s;
-  const int key_bits = st->key_bits;
-  if (key_bits == 0) return;
-  const uint32_t* keys = vg_sorted_in_a(key_bits) ? ka : kb;
-  // voxels that start in earlier tiles
-  uint32_t part = 0;
-  for (uint32_t b = threadIdx.x; b < blockIdx.x; b += 256) part += tile_cnt[b];
-  uint32_t pre;
-  block_excl_scan<256>(part, &pre, sm);
-  if (threadIdx.x == 0) pre_s = pre;
-  uint32_t c;
-  const uint32_t base = blockIdx.x * VG_TILE + threadIdx.x * 8;
-  const uint32_t bits = vg_head_flags8(keys, base, n, st->sentinel, &c);
-  uint32_t tot;
-  uint32_t s = block_excl_scan<256>(c, &tot, sm) + pre_s;
-#pragma unroll
-  for (int j = 0; j < 8; j++)
-    if (bits & (1u << j)) seg_start[s++] = base + j;
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) { st->n_seg = pre_s + tot; st->n_final = pre_s + tot; }
-}
-
-// keep[s] = 1 iff voxel s holds >= min_points points
-__global__ void __launch_bounds__(256)
-vg_keep_kernel(const uint32_t* __restrict__ ka, const uint32_t* __restrict__ kb, const uint32_t* __restrict__ seg_start,
-               const VoxState* __restrict__ st, uint32_t n, int min_points, uint32_t* __restrict__ keep) {
-  uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t* keys = vg_sorted_in_a(st->key_bits) ? ka : kb;
-  uint32_t n_seg = st->n_seg;
-  if (s >= n_seg) { if (s < n) keep[s] = 0; return; }
-  uint32_t a = seg_start[s];
-  uint32_t k = keys[a];
-  uint32_t e = a + 1;
-  while (e < n && keys[e] == k) e++;
-  keep[s] = ((int)(e - a) >= min_points) ? 1u : 0u;
-}
-
-// The common record layout (x, y, z, intensity averaged: 16-byte records).  A warp owns 32 consecutive voxels, i.e.
-// ONE contiguous range of sorted positions: the warp stages the records of that range in shared memory (the packed
-// float4 records written by vg_keys_kernel, fetched through the sorted point numbers: 16-byte gathers from an
-// L2-resident array), and every lane then adds up its own voxel's records from shared memory in ascending input order
-// (the order defines the float32 rounding) -- no per-lane chains of dependent global loads.
-constexpr int VG4_TILE = 256;       // records per warp tile (4 KB)
-__global__ void __launch_bounds__(128)
-vg_centroid4_kernel(const __grid_constant__ VoxInputs in, uint32_t stride, const uint32_t* __restrict__ ka, const uint32_t* __restrict__ kb,
-                    const uint32_t* __restrict__ va, const uint32_t* __restrict__ vb, const float4* __restrict__ rec,
-                    const uint32_t* __restrict__ seg_start, const VoxState* __restrict__ st,
-                    const uint32_t* __restrict__ slot /*nullable*/, const uint32_t* __restrict__ keep /*nullable*/,
-                    uint32_t n, VoxelFieldsDev F, uint32_t capacity, int vec32, uint8_t* __restrict__ out,
-                    int32_t* __restrict__ out_voxel_idx) {
-  __shared__ float4 tile[4][VG4_TILE];
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const uint32_t n_seg = st->n_seg;
-  const uint32_t s0 = (blockIdx.x * 4 + wib) * 32;
-  if (s0 >= n_seg) return;                                  // whole warp
-  const bool in_a = vg_sorted_in_a(st->key_bits);
+  if (key_bits == 0) {                       // empty input or overflow: only the state goes back
+    if (blockIdx.x == 0 && threadIdx.x == 0) { VoxState s = *st; s.n_final = 0; *h_st = s; }
+    return;
+  }
+  if (threadIdx.x == 0) tile_sm = atomicAdd(&st->seg_ticket, 1u);
+  __syncthreads();
+  const uint32_t tile = tile_sm;
+  const bool in_a = vg_sorted_in_a(key_bits);
   const uint32_t* keys = in_a ? ka : kb;
   const uint32_t* vals = in_a ? va : vb;
-  const uint32_t s = s0 + lane;
-  const bool seg = s < n_seg;
-  uint32_t a = 0, e = 0, k = 0;
-  if (seg) {
-    a = seg_start[s];
-    k = keys[a];
-    // segment end: next segment's start, or the first sentinel key after the last voxel
-    if (s + 1 < n_seg) e = seg_start[s + 1];
-    else { e = a + 1; while (e < n && keys[e] == k) e++; }
-  }
-  const uint32_t n_act = min(32u, n_seg - s0);
-  const uint32_t r0 = __shfl_sync(0xffffffffu, a, 0);
-  const uint32_t r1 = __shfl_sync(0xffffffffu, e, (int)n_act - 1);
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (uint32_t t0 = r0; t0 < r1; t0 += VG4_TILE) {
-    const uint32_t t1 = min(r1, t0 + (uint32_t)VG4_TILE);
-    // a tile is 8 records per lane: all 8 point numbers, then all 8 records, are in flight at once (a loop of
-    // load -> store pairs would expose one memory latency per record)
-    {
-      uint32_t pv[VG4_TILE / 32];
-      float4 rv[VG4_TILE / 32];
+  const uint32_t sentinel = st->sentinel;
+  const uint32_t t0 = tile * VG_SEG_TILE, t1 = min(n, t0 + VG_SEG_TILE);
+  // 1.
+  uint32_t nb;
+  {
+    const uint32_t base = t0 + threadIdx.x * 4;
+    uint32_t bits = 0, c = 0;
+    uint32_t prev = (base > 0 && base <= n) ? keys[base - 1] : 0xffffffffu;
 #pragma unroll
-      for (int u = 0; u < VG4_TILE / 32; u++) {
-        const uint32_t i = t0 + lane + 32u * u;
-        pv[u] = (i < t1) ? vals[i] : 0xffffffffu;
+    for (int j = 0; j < 4; j++) {
+      const uint32_t i = base + j;
+      if (i < n) {
+        const uint32_t k = keys[i];
+        if (i == 0 || k != prev) { bits |= 1u << j; c++; }
+        prev = k;
       }
-#pragma unroll
-      for (int u = 0; u < VG4_TILE / 32; u++) rv[u] = (pv[u] != 0xffffffffu) ? rec[pv[u]] : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int u = 0; u < VG4_TILE / 32; u++) tile[wib][lane + 32 * u] = rv[u];
     }
-    __syncwarp();
-    if (seg) {
-      uint32_t lo = max(a, t0), hi = min(e, t1);
-      if (lo < hi && lo == a) { acc = tile[wib][lo - t0]; lo++; }      // the sum starts from the first record itself
-      for (; lo + 4 <= hi; lo += 4) {
-        const float4 v0 = tile[wib][lo - t0], v1 = tile[wib][lo + 1 - t0], v2 = tile[wib][lo + 2 - t0], v3 = tile[wib][lo + 3 - t0];
+    uint32_t q = block_excl_scan<256>(c, &nb, scan_sm);
+#pragma unroll
+    for (int j = 0; j < 4; j++)
+      if (bits & (1u << j)) bnd[q++] = base + j;
+  }
+  __syncthreads();
+  // 2.
+  if (threadIdx.x < 32) {
+    uint32_t e = t1;
+    if (nb > 0 && t1 < n) {
+      const uint32_t k = keys[bnd[nb - 1]];
+      if (k < sentinel) {
+        for (;; e += 32) {
+          const uint32_t i = e + threadIdx.x;
+          const uint32_t other = __ballot_sync(0xffffffffu, !(i < n && keys[i] == k));
+          if (other) { e += __ffs(other) - 1; break; }
+        }
+      }
+    }
+    if (threadIdx.x == 0) tail_sm = e;
+  }
+  __syncthreads();
+  const uint32_t tail = tail_sm;
+  const uint32_t staged = min(tail, t0 + 2 * VG_SEG_TILE);
+  // 3.
+  if (FOUR) {
+    uint32_t pv[2 * VG_SEG_TILE / 256];
+    float4 rv[2 * VG_SEG_TILE / 256];
+#pragma unroll
+    for (int u = 0; u < 2 * VG_SEG_TILE / 256; u++) {
+      const uint32_t i = t0 + threadIdx.x + 256u * u;
+      pv[u] = (i < staged) ? vals[i] : 0xffffffffu;
+    }
+#pragma unroll
+    for (int u = 0; u < 2 * VG_SEG_TILE / 256; u++) rv[u] = (pv[u] != 0xffffffffu) ? rec[pv[u]] : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int u = 0; u < 2 * VG_SEG_TILE / 256; u++)
+      if (pv[u] != 0xffffffffu) recs[threadIdx.x + 256u * u] = rv[u];
+  }
+  for (uint32_t h = threadIdx.x; h < nb; h += 256) {
+    const uint32_t a = bnd[h];
+    const uint32_t k = keys[a];
+    uint32_t e = 0;
+    if (k < sentinel) {
+      e = (h + 1 < nb) ? bnd[h + 1] : tail;
+      if (min_points > 1 && (int)(e - a) < min_points) e = 0;
+    }
+    endp[h] = e;
+  }
+  __syncthreads();
+  // 4.
+  {
+    uint32_t kc = 0;
+#pragma unroll
+    for (int j = 0; j < 4; j++) { const uint32_t h = threadIdx.x * 4 + j; if (h < nb && endp[h]) kc++; }
+    uint32_t tot;
+    uint32_t r = block_excl_scan<256>(kc, &tot, scan_sm);
+#pragma unroll
+    for (int j = 0; j < 4; j++) { const uint32_t h = threadIdx.x * 4 + j; if (h < nb && endp[h]) slot[h] = r++; }
+    if (threadIdx.x < 32) {
+      uint32_t* mine = seg_status + tile;
+      if (threadIdx.x == 0) lookback_publish(mine, tile == 0 ? (LB_PREFIX | tot) : tot);
+      const uint32_t pre = tile == 0 ? 0u : lookback_prefix_warp(seg_status, tile);
+      if (threadIdx.x == 0 && tile > 0) lookback_publish(mine, LB_PREFIX | (pre + tot));
+      if (threadIdx.x == 0) pre_sm = pre;
+      if (threadIdx.x == 0 && tile == gridDim.x - 1) {           // every earlier tile is counted: the call's result is known
+        st->n_final = pre + tot;
+        VoxState s = *st;
+        s.n_final = pre + tot;
+        *h_st = s;
+      }
+    }
+  }
+  __syncthreads();
+  // 5.
+  const uint32_t pre = pre_sm;
+  for (uint32_t h = threadIdx.x; h < nb; h += 256) {
+    const uint32_t e = endp[h];
+    if (!e) continue;
+    const uint32_t o = pre + slot[h];
+    if (o >= capacity) continue;
+    const uint32_t a = bnd[h];
+    int cfirst;
+    const uint8_t* first = vg_point(in, vals[a], stride, cfirst);
+    uint8_t* dst = out + (size_t)o * stride;
+    const float cnt = (float)(e - a);
+    if (FOUR) {
+      float4 acc = recs[a - t0];                                  // the sum starts from the first record itself
+      const uint32_t em = min(e, staged);
+      uint32_t j = a + 1;
+      for (; j < em; j++) {
+        const float4 v = recs[j - t0];
+        acc.x = acc.x + v.x; acc.y = acc.y + v.y; acc.z = acc.z + v.z; acc.w = acc.w + v.w;
+      }
+      for (; j + 4 <= e; j += 4) {                                // past the staged records: 4 gathers in flight, added in order
+        const uint32_t p0 = vals[j], p1 = vals[j + 1], p2 = vals[j + 2], p3 = vals[j + 3];
+        const float4 v0 = rec[p0], v1 = rec[p1], v2 = rec[p2], v3 = rec[p3];
         acc.x = acc.x + v0.x; acc.y = acc.y + v0.y; acc.z = acc.z + v0.z; acc.w = acc.w + v0.w;
         acc.x = acc.x + v1.x; acc.y = acc.y + v1.y; acc.z = acc.z + v1.z; acc.w = acc.w + v1.w;
         acc.x = acc.x + v2.x; acc.y = acc.y + v2.y; acc.z = acc.z + v2.z; acc.w = acc.w + v2.w;
         acc.x = acc.x + v3.x; acc.y = acc.y + v3.y; acc.z = acc.z + v3.z; acc.w = acc.w + v3.w;
       }
-      for (; lo < hi; lo++) {
-        const float4 v = tile[wib][lo - t0];
+      for (; j < e; j++) {
+        const float4 v = rec[vals[j]];
         acc.x = acc.x + v.x; acc.y = acc.y + v.y; acc.z = acc.z + v.z; acc.w = acc.w + v.w;
       }
+      // bytes not covered by an averaged field come from the voxel's first point
+      if (vec32 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0) {
+        const uint4 w0 = reinterpret_cast<const uint4*>(first)[0], w1 = reinterpret_cast<const uint4*>(first)[1];
+        reinterpret_cast<uint4*>(dst)[0] = w0; reinterpret_cast<uint4*>(dst)[1] = w1;
+      } else {
+        for (uint32_t w = 0; w < stride / 4; w++)
+          reinterpret_cast<uint32_t*>(dst)[w] = reinterpret_cast<const uint32_t*>(first)[w];
+      }
+      *reinterpret_cast<float*>(dst + F.ff_off[0]) = acc.x / cnt;
+      *reinterpret_cast<float*>(dst + F.ff_off[1]) = acc.y / cnt;
+      *reinterpret_cast<float*>(dst + F.ff_off[2]) = acc.z / cnt;
+      *reinterpret_cast<float*>(dst + F.ff_off[3]) = acc.w / cnt;
+    } else {
+      float acc[VG_MAX_FIELDS];
+      const int nf = F.n_ff;
+#pragma unroll
+      for (int f = 0; f < VG_MAX_FIELDS; f++) acc[f] = (f < nf) ? *reinterpret_cast<const float*>(first + F.ff_off[f]) : 0.f;
+      for (uint32_t j = a + 1; j < e; j++) {
+        int cj;
+        const uint8_t* p = vg_point(in, vals[j], stride, cj);
+#pragma unroll
+        for (int f = 0; f < VG_MAX_FIELDS; f++)
+          if (f < nf) acc[f] = acc[f] + *reinterpret_cast<const float*>(p + F.ff_off[f]);
+      }
+      // bytes not covered by an averaged field come from the voxel's first point
+      for (uint32_t w = 0; w < stride / 4; w++)
+        reinterpret_cast<uint32_t*>(dst)[w] = reinterpret_cast<const uint32_t*>(first)[w];
+#pragma unroll
+      for (int f = 0; f < VG_MAX_FIELDS; f++)
+        if (f < nf) *reinterpret_cast<float*>(dst + F.ff_off[f]) = acc[f] / cnt;
     }
-    __syncwarp();
+    if (out_voxel_idx) out_voxel_idx[o] = (int32_t)keys[a];
   }
-  if (!seg) return;
-  if (keep && !keep[s]) return;
-  const uint32_t o = slot ? slot[s] : s;
-  if (o >= capacity) return;
-  const float cnt = (float)(e - a);
-  int cfirst;
-  const uint8_t* first = vg_point(in, vals[a], stride, cfirst);
-  uint8_t* dst = out + (size_t)o * stride;
-  // bytes not covered by an averaged field come from the voxel's first point
-  if (vec32 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0) {
-    const uint4 w0 = reinterpret_cast<const uint4*>(first)[0], w1 = reinterpret_cast<const uint4*>(first)[1];
-    reinterpret_cast<uint4*>(dst)[0] = w0; reinterpret_cast<uint4*>(dst)[1] = w1;
-  } else {
-    for (uint32_t w = 0; w < stride / 4; w++)
-      reinterpret_cast<uint32_t*>(dst)[w] = reinterpret_cast<const uint32_t*>(first)[w];
-  }
-  *reinterpret_cast<float*>(dst + F.ff_off[0]) = acc.x / cnt;
-  *reinterpret_cast<float*>(dst + F.ff_off[1]) = acc.y / cnt;
-  *reinterpret_cast<float*>(dst + F.ff_off[2]) = acc.z / cnt;
-  *reinterpret_cast<float*>(dst + F.ff_off[3]) = acc.w / cnt;
-  if (out_voxel_idx) out_voxel_idx[o] = (int32_t)k;
-}
-
-// Any other set of averaged fields: one thread per voxel, float32 sum of its points in ascending input order (the order
-// the stable sort produced), read straight from the caller's layout through the sorted point numbers; divide by the
-// count (centroid /= float(n), PCL), write the output point.
-__global__ void __launch_bounds__(128)
-vg_centroid_kernel(const uint8_t* __restrict__ in, uint32_t stride, const uint32_t* __restrict__ ka, const uint32_t* __restrict__ kb,
-                   const uint32_t* __restrict__ va, const uint32_t* __restrict__ vb,
-                   const uint32_t* __restrict__ seg_start, const VoxState* __restrict__ st,
-                   const uint32_t* __restrict__ slot /*nullable*/, const uint32_t* __restrict__ keep /*nullable*/,
-                   uint32_t n, VoxelFieldsDev F, uint32_t capacity, uint8_t* __restrict__ out,
-                   int32_t* __restrict__ out_voxel_idx) {
-  uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t n_seg = st->n_seg;
-  if (s >= n_seg) return;
-  if (keep && !keep[s]) return;
-  uint32_t o = slot ? slot[s] : s;
-  if (o >= capacity) return;
-  const bool in_a = vg_sorted_in_a(st->key_bits);
-  const uint32_t* keys = in_a ? ka : kb;
-  const uint32_t* vals = in_a ? va : vb;
-  uint32_t a = seg_start[s];
-  uint32_t k = keys[a];
-  // segment end: next segment's start, or the first sentinel key after the last voxel
-  uint32_t e;
-  if (s + 1 < n_seg) e = seg_start[s + 1];
-  else { e = a + 1; while (e < n && keys[e] == k) e++; }
-  float acc[VG_MAX_FIELDS];
-  const int nf = F.n_ff;
-  const uint8_t* first = in + (size_t)vals[a] * stride;
-#pragma unroll
-  for (int f = 0; f < VG_MAX_FIELDS; f++) acc[f] = (f < nf) ? *reinterpret_cast<const float*>(first + F.ff_off[f]) : 0.f;
-  for (uint32_t j = a + 1; j < e; j++) {
-    const uint8_t* p = in + (size_t)vals[j] * stride;
-#pragma unroll
-    for (int f = 0; f < VG_MAX_FIELDS; f++)
-      if (f < nf) acc[f] = acc[f] + *reinterpret_cast<const float*>(p + F.ff_off[f]);
-  }
-  float cnt = (float)(e - a);
-  uint8_t* dst = out + (size_t)o * stride;
-  // bytes not covered by an averaged field come from the voxel's first point
-  for (uint32_t w = 0; w < stride / 4; w++)
-    reinterpret_cast<uint32_t*>(dst)[w] = reinterpret_cast<const uint32_t*>(first)[w];
-#pragma unroll
-  for (int f = 0; f < VG_MAX_FIELDS; f++)
-    if (f < nf) *reinterpret_cast<float*>(dst + F.ff_off[f]) = acc[f] / cnt;
-  if (out_voxel_idx) out_voxel_idx[o] = (int32_t)k;
 }
 
 __global__ void vg_state_init_kernel(VoxState* st) {
   if (threadIdx.x == 0) {
     bbox_reset(&st->acc);
-    st->ticket = 0; st->status = 0; st->sentinel = 0; st->key_bits = 0; st->count = 0; st->n_seg = 0; st->n_final = 0;
+    st->ticket = 0; st->seg_ticket = 0; st->status = 0; st->sentinel = 0; st->key_bits = 0; st->count = 0; st->n_final = 0;
     for (int d = 0; d < 3; d++) { st->min_b[d] = 0; st->div_b[d] = 0; }
   }
 }
@@ -504,13 +539,12 @@ struct lb_voxel {
   int pass_negative = 0;
   DBuf<uint8_t> d_in, d_out;
   DBuf<int32_t> d_vidx;
-  DBuf<uint32_t> keys, tile_cnt, seg_start, keep, slot;
+  DBuf<uint32_t> keys, seg_status;
   DBuf<float4> rec;
   VoxState* d_st = nullptr;     // device
-  VoxState* h_st = nullptr;     // pinned
+  VoxState* h_st = nullptr;     // pinned, written by vg_segment_kernel
   int bits_hint = 32;           // sort passes to enqueue: the key width of the previous call, rounded up to whole passes
   SortWork sort;
-  ScanWork scan;
   FeatWork* feat = nullptr;     // created by the first lb_voxel_extract_features
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   float t_last_ms = 0.f;
@@ -545,10 +579,8 @@ int lb_voxel_destroy(lb_voxel* h) {
   if (!h) return LB_OK;
   cudaSetDevice(h->c.device);
   cudaStreamSynchronize(h->c.stream);
-  h->d_in.release(); h->d_out.release(); h->d_vidx.release(); h->keys.release(); h->tile_cnt.release();
-  h->seg_start.release(); h->keep.release(); h->slot.release(); h->rec.release();
-  h->sort.ka.release(); h->sort.kb.release(); h->sort.va.release(); h->sort.vb.release(); h->sort.hist.release();
-  h->sort.scan.sums.release(); h->scan.sums.release();
+  h->d_in.release(); h->d_out.release(); h->d_vidx.release(); h->keys.release(); h->seg_status.release(); h->rec.release();
+  h->sort.ka.release(); h->sort.kb.release(); h->sort.va.release(); h->sort.vb.release(); h->sort.state.release();
   feat_work_free(h->feat);
   if (h->d_st) cudaFree(h->d_st);
   if (h->h_st) cudaFreeHost(h->h_st);
@@ -739,8 +771,9 @@ static int voxel_filter_impl(lb_voxel* h, const lb_voxel_input* inputs, int n_in
     d_out = h->d_out.p; capacity = n;
     if (out_voxel_idx) { LB_TRY(h->d_vidx.ensure(n)); d_vidx = h->d_vidx.p; }
   }
-  const uint32_t ntiles = (uint32_t)cdiv(n, VG_TILE);
-  LB_TRY(h->keys.ensure(n)); LB_TRY(h->seg_start.ensure(n)); LB_TRY(h->tile_cnt.ensure(ntiles));
+  const uint32_t seg_tiles = (uint32_t)cdiv(n, VG_SEG_TILE);
+  LB_TRY(h->keys.ensure(n)); LB_TRY(h->seg_status.ensure(seg_tiles));
+  LB_TRY(radix_sort_reserve(c, h->sort, n));
   const bool four = F.n_ff == 4;
   if (four) LB_TRY(h->rec.ensure(n));
   if (!four && (n_inputs > 1 || any_T)) {
@@ -754,7 +787,6 @@ static int voxel_filter_impl(lb_voxel* h, const lb_voxel_input* inputs, int n_in
   // 32-byte records on 16-byte aligned bases: two 16-byte loads per point instead of 4-byte strided ones
   int vec32 = point_step == 32 ? 1 : 0;
   for (int i = 0; i < n_inputs; i++) if (reinterpret_cast<uintptr_t>(vin.base[i]) & 15u) vec32 = 0;
-  const uint8_t* d_in = vin.base[0];
   VoxLimits lim;
   lim.ff_off = ffo; lim.fmin = (float)h->lim_min; lim.fmax = (float)h->lim_max; lim.dmin = h->lim_min; lim.dmax = h->lim_max;
   lim.negative = h->negative;
@@ -763,36 +795,25 @@ static int voxel_filter_impl(lb_voxel* h, const lb_voxel_input* inputs, int n_in
   // box, i.e. it is known on the device only; passes are enqueued for the width the previous call needed (consecutive
   // scans of a stream have the same extent), passes beyond the actual width return at once, and in the rare case that
   // this call needs MORE passes than were enqueued the chain is simply run again with all four.
-  const uint32_t *ka = nullptr, *kb = nullptr, *va = nullptr, *vb = nullptr;
   for (int attempt = 0; attempt < 2; attempt++) {
     const int launched_bits = attempt == 0 ? h->bits_hint : 32;
     const int bb_blocks = min(cdiv(n, 256), c.sm_count * 4);
     vg_bbox_kernel<<<bb_blocks, 256, 0, c.stream>>>(vin, n, point_step, (uint32_t)xo, lim, h->body, inv0, inv1, inv2, vec32, h->d_st);
-    vg_keys_kernel<<<cdiv(n, 256), 256, 0, c.stream>>>(vin, n, point_step, (uint32_t)xo, lim, h->body, inv0, inv1, inv2, vec32, F,
-                                                       h->d_st, h->keys.p, four ? h->rec.p : nullptr);
+    vg_keys_kernel<<<cdiv(n, 256 * VG_KEYS_ITEMS), 256, 0, c.stream>>>(vin, n, point_step, (uint32_t)xo, lim, h->body, inv0, inv1, inv2,
+                                                                        vec32, F, h->d_st, h->keys.p, four ? h->rec.p : nullptr,
+                                                                        h->sort.dev(), h->sort.status(), rs_tiles(n),
+                                                                        h->seg_status.p, seg_tiles);
     c.launches += 2;
     LB_TRY(radix_sort_pairs_devbits(c, h->sort, h->keys.p, n, launched_bits, &h->d_st->key_bits));
-    ka = h->sort.ka.p; kb = h->sort.kb.p; va = h->sort.va.p; vb = h->sort.vb.p;
-    vg_tile_heads_kernel<<<ntiles, 256, 0, c.stream>>>(ka, kb, h->d_st, n, h->tile_cnt.p);
-    vg_segstart_kernel<<<ntiles, 256, 0, c.stream>>>(ka, kb, h->d_st, n, h->tile_cnt.p, h->seg_start.p);
-    c.launches += 2;
-    const uint32_t* slot = nullptr; const uint32_t* keep = nullptr;
-    if (h->min_points > 1) {
-      LB_TRY(h->keep.ensure(n)); LB_TRY(h->slot.ensure(n));
-      vg_keep_kernel<<<cdiv(n, 256), 256, 0, c.stream>>>(ka, kb, h->seg_start.p, h->d_st, n, h->min_points, h->keep.p);
-      c.launches++;
-      LB_TRY(exclusive_scan_u32(c, h->scan, h->keep.p, h->slot.p, n, &h->d_st->n_final));
-      slot = h->slot.p; keep = h->keep.p;
-    }
+    const uint32_t *ka = h->sort.ka.p, *kb = h->sort.kb.p, *va = h->sort.va.p, *vb = h->sort.vb.p;
     if (four)
-      vg_centroid4_kernel<<<cdiv(n, 128), 128, 0, c.stream>>>(vin, point_step, ka, kb, va, vb, h->rec.p, h->seg_start.p, h->d_st,
-                                                               slot, keep, n, F, capacity, vec32, d_out, d_vidx);
+      vg_segment_kernel<true><<<seg_tiles, 256, 0, c.stream>>>(vin, point_step, ka, kb, va, vb, h->rec.p, h->d_st, h->h_st, h->seg_status.p,
+                                                              n, h->min_points, F, capacity, vec32, d_out, d_vidx);
     else
-      vg_centroid_kernel<<<cdiv(n, 128), 128, 0, c.stream>>>(d_in, point_step, ka, kb, va, vb, h->seg_start.p, h->d_st, slot, keep,
-                                                              n, F, capacity, d_out, d_vidx);
+      vg_segment_kernel<false><<<seg_tiles, 256, 0, c.stream>>>(vin, point_step, ka, kb, va, vb, nullptr, h->d_st, h->h_st, h->seg_status.p,
+                                                               n, h->min_points, F, capacity, vec32, d_out, d_vidx);
     c.launches++;
     LB_CUDA(cudaGetLastError());
-    LB_CUDA(cudaMemcpyAsync(h->h_st, h->d_st, sizeof(VoxState), cudaMemcpyDeviceToHost, c.stream));
     if (mem_out != LB_MEM_HOST) LB_CUDA(cudaEventRecord(h->ev1, c.stream));
     LB_CUDA(cudaStreamSynchronize(c.stream));        // the one synchronisation of a device-to-device call
     if (h->h_st->key_bits <= launched_bits) break;   // every pass the key needs was enqueued
