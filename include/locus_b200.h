@@ -532,6 +532,29 @@ int lb_odometry_set_normals(lb_odometry* h, int k, const float* viewpoint);
 int lb_odometry_submit(lb_odometry* h, const uint8_t* scan, size_t n_pts, uint32_t point_step, const lb_field* fields,
                        int n_fields, int mem, const float* guess, uint8_t* filtered_out, int mem_filtered,
                        uint64_t* ticket);
+/* One scan of a robot with several lidars: the stage-V work of the front-end nodes in LOCUS's multi-lidar launch (one
+ * pcl/PassThrough per lidar, point_cloud_merger, BodyFilter, VoxelGrid) as one lb_voxel_filter_merged call on the
+ * pipeline's voxel handle, in place of lb_voxel_filter.  Everything after the VoxelGrid is that of lb_odometry_submit;
+ * the filtered scan (and, with lb_locus, the keyframe the map receives) is the merged one.
+ *   Order: inputs[0 .. n_inputs-1] are merged in the order given, as lb_voxel_filter_merged does.  Inside a voxel the
+ *     points are summed in merged order, so the order changes the centroids' bits: pass the merger's alive_keys_ order
+ *     (PointCloudMerger.cc:191-250; a lidar that failed and came back is last).
+ *   Varying count: n_inputs (1..3) may change from one scan to the next, and an input may have n_pts = 0.  A scan whose
+ *     inputs are all empty filters to nothing and changes no state, as an empty scan does.
+ *   Lifetimes: every input's data must stay valid until the scan's result is returned (as `scan` above).  The
+ *     transforms (row-major 4x4 float, sensor -> base_link; NULL = identity) are copied here, so they may live on the
+ *     caller's stack.
+ *   Settings: PassThrough, BodyFilter, limits and leaf come from the pipeline's voxel handle (lb_odometry_voxel /
+ *     lb_locus_voxel), as for one cloud; lb_locus's adaptive voxelization retunes on the merged filtered count.
+ *   Refused here (no ticket taken, pending unchanged): n_inputs outside 1..3, inputs NULL, data NULL with n_pts > 0
+ *     (LB_ERR_INVALID_ARG); sum of n_pts > max_points or point_step > max_point_step (LB_ERR_CAPACITY).
+ *   What lb_voxel_filter_merged itself refuses (a layout other than x, y, z, intensity with more than one input or with
+ *     a transform: LB_ERR_UNSUPPORTED) comes back as the scan's result status and changes no state, like any failed
+ *     VoxelGrid.
+ *   filtered_out (nullable) must hold sum(n_pts) * point_step bytes. */
+int lb_odometry_submit_merged(lb_odometry* h, const lb_voxel_input* inputs, int n_inputs, uint32_t point_step,
+                              const lb_field* fields, int n_fields, int mem, const float* guess,
+                              uint8_t* filtered_out, int mem_filtered, uint64_t* ticket);
 /* next result in submission order.  block != 0: wait for it; block == 0: returns 1 when it is not ready yet.
  * Returns LB_ERR_NO_ALIGN when every submitted scan has already been returned. */
 int lb_odometry_next(lb_odometry* h, lb_odometry_result* r, int block);
@@ -647,6 +670,11 @@ int lb_locus_set_params(lb_locus* h, const lb_locus_params* p);
 /* same arguments and blocking rule as lb_odometry_submit; guess = the odometry prior */
 int lb_locus_submit(lb_locus* h, const uint8_t* scan, size_t n_pts, uint32_t point_step, const lb_field* fields,
                     int n_fields, int mem, const float* guess, uint8_t* filtered_out, int mem_filtered, uint64_t* ticket);
+/* same arguments and rules as lb_odometry_submit_merged (order, varying lidar count, lifetimes, copied transforms,
+ * refusals): one scan of 1..3 lidars merged in the VoxelGrid stage; the keyframe inserted is the merged filtered scan */
+int lb_locus_submit_merged(lb_locus* h, const lb_voxel_input* inputs, int n_inputs, uint32_t point_step,
+                           const lb_field* fields, int n_fields, int mem, const float* guess, uint8_t* filtered_out,
+                           int mem_filtered, uint64_t* ticket);
 int lb_locus_next(lb_locus* h, lb_locus_result* r, int block);
 int lb_locus_pending(lb_locus* h, size_t* n);
 /* out9 = the six values of lb_odometry_stage_times, then { scans localized, localization stage busy s, its wait s } */

@@ -155,9 +155,9 @@ SYMBOLS = [
     "lb_submap_generation", "lb_submap_points", "lb_submap_insert_with_normals", "lb_submap_normals", "lb_submap_neighbors", "lb_submap_launch_count", "lb_gicp_set_target_submap",
     "lb_odometry_create", "lb_odometry_destroy", "lb_odometry_voxel", "lb_odometry_gicp", "lb_odometry_depth",
     "lb_odometry_set_gicp_params", "lb_odometry_set_cloud_sharing", "lb_odometry_set_normals", "lb_odometry_submit", "lb_odometry_next", "lb_odometry_pending",
-    "lb_odometry_launch_count", "lb_odometry_stage_times",
+    "lb_odometry_launch_count", "lb_odometry_stage_times", "lb_odometry_submit_merged",
     "lb_locus_default_params", "lb_locus_create", "lb_locus_destroy", "lb_locus_voxel", "lb_locus_set_params", "lb_locus_submit",
-    "lb_locus_next", "lb_locus_pending", "lb_locus_stage_times",
+    "lb_locus_next", "lb_locus_pending", "lb_locus_stage_times", "lb_locus_submit_merged",
     "lb_ndt_default_params", "lb_ndt_create", "lb_ndt_create_on_stream", "lb_ndt_destroy", "lb_ndt_set_params", "lb_ndt_set_source",
     "lb_ndt_set_target", "lb_ndt_align", "lb_ndt_target_voxels", "lb_ndt_derivatives", "lb_ndt_launch_count",
 ]
@@ -288,6 +288,9 @@ def lib():
         L.lb_odometry_pending.argtypes = [vp, C.POINTER(sz)]
         L.lb_odometry_launch_count.argtypes = [vp, u64p]
         L.lb_odometry_stage_times.argtypes = [vp, C.POINTER(C.c_double)]
+        if hasattr(L, "lb_odometry_submit_merged"):
+            L.lb_odometry_submit_merged.argtypes = [vp, C.POINTER(VoxelInput), i32, C.c_uint32, C.POINTER(Field), i32, i32, vp, vp,
+                                                    i32, u64p]
     if hasattr(L, "lb_locus_create"):
         L.lb_locus_default_params.argtypes = [C.POINTER(LocusParams)]
         L.lb_locus_create.argtypes = [i32, i32, sz, C.c_uint32, vp, C.POINTER(vp)]
@@ -298,6 +301,9 @@ def lib():
         L.lb_locus_next.argtypes = [vp, C.POINTER(LocusResult), i32]
         L.lb_locus_pending.argtypes = [vp, C.POINTER(sz)]
         L.lb_locus_stage_times.argtypes = [vp, C.POINTER(C.c_double)]
+        if hasattr(L, "lb_locus_submit_merged"):
+            L.lb_locus_submit_merged.argtypes = [vp, C.POINTER(VoxelInput), i32, C.c_uint32, C.POINTER(Field), i32, i32, vp, vp,
+                                                 i32, u64p]
     if hasattr(L, "lb_ndt_create"):
         L.lb_ndt_default_params.argtypes = [C.POINTER(NdtParams)]
         L.lb_ndt_default_params.restype = None
@@ -338,6 +344,30 @@ def _ptr(a):
 def xyzi_fields():
     """PointField list of pcl::PointXYZI as it leaves BodyFilter (body_filter.cc:36-39)."""
     return [("x", 0, LB_FLOAT32, 1), ("y", 4, LB_FLOAT32, 1), ("z", 8, LB_FLOAT32, 1), ("intensity", 16, LB_FLOAT32, 1)]
+
+
+def _merged_inputs(blobs, point_step, transforms):
+    """lb_voxel_input[] for 1..3 clouds: each a host uint8 numpy array (n = size // point_step) or a (pointer, n_pts)
+    pair (a device cloud); transforms: None or one 4x4 (or None) per cloud.  Returns (array, what must stay alive)."""
+    transforms = [None] * len(blobs) if transforms is None else list(transforms)
+    if len(transforms) != len(blobs):
+        raise ValueError("one transform (or None) per cloud")
+    arr = (VoxelInput * max(len(blobs), 1))()
+    keep = []
+    for i, (b, T) in enumerate(zip(blobs, transforms)):
+        if isinstance(b, tuple):
+            arr[i].data = int(b[0]) or None
+            arr[i].n_pts = int(b[1])
+        else:
+            b = np.ascontiguousarray(b, dtype=np.uint8).reshape(-1)
+            arr[i].data = b.ctypes.data_as(C.c_void_p).value
+            arr[i].n_pts = b.size // point_step
+        keep.append(b)
+        if T is not None:
+            T = np.ascontiguousarray(T, dtype=np.float32).reshape(16)      # the library copies it at submit
+            arr[i].transform = T.ctypes.data_as(C.c_void_p).value
+            keep.append(T)
+    return arr, keep
 
 
 class GicpB200:
@@ -921,6 +951,20 @@ class OdometryB200:
         self._keep[t.value] = (scan, fa, g, filtered_out)        # buffers stay alive until the result is returned
         return t.value
 
+    def submit_merged(self, blobs, point_step, fields, transforms=None, mem=LB_MEM_HOST, guess=None, filtered_out=None,
+                      mem_filtered=LB_MEM_HOST):
+        """one scan of 1..3 lidars merged in the VoxelGrid stage (lb_odometry_submit_merged), in the order given (the
+        merger's alive_keys_ order); blobs: host uint8 numpy arrays or (pointer, n_pts) pairs; transforms: one 4x4
+        sensor -> base_link (or None) per cloud.  filtered_out holds sum(n_pts) * point_step bytes.  Returns the ticket."""
+        fa = fields if not isinstance(fields, (list, tuple)) else VoxelGridB200._fields(fields)
+        arr, keep = _merged_inputs(blobs, point_step, transforms)
+        t = C.c_uint64(0)
+        g = None if guess is None else np.ascontiguousarray(guess, dtype=np.float32).reshape(16)
+        _check(lib().lb_odometry_submit_merged(self._h, arr, len(blobs), point_step, fa, len(fa), mem, _ptr(g),
+                                               _ptr(filtered_out), mem_filtered, C.byref(t)))
+        self._keep[t.value] = (keep, fa, g, filtered_out)         # the clouds stay alive until the result is returned
+        return t.value
+
     def next(self, block=True):
         """next result in submission order, or None when block=False and it is not ready."""
         r = OdometryResult()
@@ -1014,6 +1058,19 @@ class LocusB200:
         _check(lib().lb_locus_submit(self._h, _ptr(scan), n_pts, point_step, fa, len(fa), mem, _ptr(g),
                                      _ptr(filtered_out), mem_filtered, C.byref(t)))
         self._keep[t.value] = (scan, fa, g, filtered_out)
+        return t.value
+
+    def submit_merged(self, blobs, point_step, fields, transforms=None, mem=LB_MEM_HOST, guess=None, filtered_out=None,
+                      mem_filtered=LB_MEM_HOST):
+        """as OdometryB200.submit_merged (lb_locus_submit_merged): 1..3 lidars merged in the VoxelGrid stage; the
+        keyframe the map receives is the merged filtered scan.  Returns the ticket."""
+        fa = fields if not isinstance(fields, (list, tuple)) else VoxelGridB200._fields(fields)
+        arr, keep = _merged_inputs(blobs, point_step, transforms)
+        t = C.c_uint64(0)
+        g = None if guess is None else np.ascontiguousarray(guess, dtype=np.float32).reshape(16)
+        _check(lib().lb_locus_submit_merged(self._h, arr, len(blobs), point_step, fa, len(fa), mem, _ptr(g),
+                                            _ptr(filtered_out), mem_filtered, C.byref(t)))
+        self._keep[t.value] = (keep, fa, g, filtered_out)
         return t.value
 
     def next(self, block=True):

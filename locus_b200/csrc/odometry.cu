@@ -31,11 +31,16 @@
 #include "locus_stub.h"
 #include "front_end_stub.h"
 #include "icp_covariance_stub.h"
+#include "merged_stub.h"
 #elif defined(LB_ODOMETRY_STUB)  // TEST-ONLY build without CUDA: tests/odometry_harness.cpp supplies fake stages
 #include "odometry_stub.h"
 #include "front_end_stub.h"
+#include "merged_stub.h"
 #else
 #include "prims.cuh"
+namespace lb {
+int voxel_reserve(lb_voxel* h, size_t n_pts, uint32_t max_step);   // voxel.cu
+}
 #endif
 #include "lo_pose.h"
 
@@ -43,10 +48,19 @@ using namespace lb;
 
 namespace {
 
+constexpr int MAX_LIDARS = 3;      // lb_voxel_filter_merged's input limit
+
 struct Job {
   uint64_t ticket = 0;
   const uint8_t* scan = nullptr;
   size_t n_pts = 0;
+  // lb_odometry_submit_merged: n_inputs > 0 clouds in merge order (scan unused; n_pts = their sum), each with its
+  // transform copied at submit (has_T[i] = 0: identity)
+  int n_inputs = 0;
+  const uint8_t* in_data[MAX_LIDARS] = {nullptr, nullptr, nullptr};
+  size_t in_pts[MAX_LIDARS] = {0, 0, 0};
+  bool has_T[MAX_LIDARS] = {false, false, false};
+  float T[MAX_LIDARS][16];
   uint32_t point_step = 0;
   std::vector<lb_field> fields;
   int mem = LB_MEM_HOST;
@@ -183,8 +197,19 @@ void voxel_stage(lb_odometry* h) {
       lb_voxel_get_leaf_size(h->vg, leaf3);
       if (!h->leaf_started) { h->leaf = leaf3[0]; h->leaf_started = true; }
     }
-    int st = lb_voxel_filter(h->vg, j.scan, j.n_pts, j.point_step, j.fields.data(), (int)j.fields.size(), nullptr, 0, s.d,
-                             h->max_points, &n_out, nullptr, j.mem, LB_MEM_DEVICE);
+    int st;
+    if (j.n_inputs) {
+      // the lidars of one scan merged, transformed and filtered by one stream-ordered VoxelGrid chain (row f4)
+      lb_voxel_input in[MAX_LIDARS];
+      for (int i = 0; i < j.n_inputs; i++) {
+        in[i].data = j.in_data[i]; in[i].n_pts = j.in_pts[i]; in[i].transform = j.has_T[i] ? j.T[i] : nullptr;
+      }
+      st = lb_voxel_filter_merged(h->vg, in, j.n_inputs, j.point_step, j.fields.data(), (int)j.fields.size(), s.d,
+                                  h->max_points, &n_out, nullptr, j.mem, LB_MEM_DEVICE);
+    } else {
+      st = lb_voxel_filter(h->vg, j.scan, j.n_pts, j.point_step, j.fields.data(), (int)j.fields.size(), nullptr, 0, s.d,
+                           h->max_points, &n_out, nullptr, j.mem, LB_MEM_DEVICE);
+    }
     s.status = st; s.n = (st == LB_OK) ? n_out : 0; s.point_step = j.point_step; s.xyz_off = j.xyz_off;
     if (st != LB_OK) copy_err(s.error, sizeof(s.error));
     if (st == LB_OK && h->adaptive) adapt_leaf(h, n_out);     // a failed VoxelGrid is a callback that never ran
@@ -322,6 +347,9 @@ int odometry_create(int device, int depth, size_t max_points, uint32_t max_point
     }
   }
   if (st == LB_OK) st = lb_voxel_create_on_stream(device, h->voxel_stream, &h->vg);
+  // no device allocation in steady state: the VoxelGrid's scratch for raw scans of up to max_points points (a merged
+  // scan grows mid-stream when a lidar comes back)
+  if (st == LB_OK) st = voxel_reserve(h->vg, max_points, max_point_step);
   for (int i = 0; st == LB_OK && i < depth; i++) {
     lb_gicp* g = nullptr;
     st = lb_gicp_create(device, &g);
@@ -454,22 +482,28 @@ int lb_odometry_set_normals(lb_odometry* h, int k, const float* viewpoint) {
   return LB_OK;
 }
 
-int lb_odometry_submit(lb_odometry* h, const uint8_t* scan, size_t n_pts, uint32_t point_step, const lb_field* fields,
-                       int n_fields, int mem, const float* guess, uint8_t* filtered_out, int mem_filtered,
-                       uint64_t* ticket) {
-  if (!h || !scan || !fields || n_fields <= 0) { set_error("lb_odometry_submit: null argument"); return LB_ERR_INVALID_ARG; }
+}  // extern "C"
+
+namespace {
+
+// the checks and the queueing both submit calls share: scan of n_pts points in total; merged: the caller fills
+// the Job's inputs into *job_out before it is queued (a callback, so that a refusal allocates nothing)
+template <class Fill>
+int submit_job(lb_odometry* h, const char* who, size_t n_pts, uint32_t point_step, const lb_field* fields, int n_fields,
+               int mem, const float* guess, uint8_t* filtered_out, int mem_filtered, uint64_t* ticket, Fill fill) {
   if (n_pts > h->max_points || point_step > h->max_step) {
-    set_error("lb_odometry_submit: scan of %zu x %u bytes exceeds the pipeline's ring (%zu x %u)", n_pts, point_step,
+    set_error("%s: scan of %zu x %u bytes exceeds the pipeline's ring (%zu x %u)", who, n_pts, point_step,
               h->max_points, h->max_step);
     return LB_ERR_CAPACITY;
   }
   int xo = -1;
   for (int f = 0; f < n_fields; f++)
     if (!strcmp(fields[f].name, "x") && fields[f].datatype == LB_FLOAT32) xo = (int)fields[f].offset;
-  if (xo < 0) { set_error("lb_odometry_submit: FLOAT32 field 'x' required"); return LB_ERR_INVALID_ARG; }
+  if (xo < 0) { set_error("%s: FLOAT32 field 'x' required", who); return LB_ERR_INVALID_ARG; }
   Entry* e = new Entry;
   Job& j = e->job;
-  j.scan = scan; j.n_pts = n_pts; j.point_step = point_step; j.fields.assign(fields, fields + n_fields); j.mem = mem;
+  j.n_pts = n_pts; j.point_step = point_step; j.fields.assign(fields, fields + n_fields); j.mem = mem;
+  fill(j);
   j.has_guess = guess != nullptr;
   if (guess) memcpy(j.guess, guess, sizeof(j.guess));
   j.filtered_out = filtered_out; j.mem_filtered = mem_filtered; j.xyz_off = xo;
@@ -484,6 +518,42 @@ int lb_odometry_submit(lb_odometry* h, const uint8_t* scan, size_t n_pts, uint32
   }
   h->cv.notify_all();
   return LB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int lb_odometry_submit(lb_odometry* h, const uint8_t* scan, size_t n_pts, uint32_t point_step, const lb_field* fields,
+                       int n_fields, int mem, const float* guess, uint8_t* filtered_out, int mem_filtered,
+                       uint64_t* ticket) {
+  if (!h || !scan || !fields || n_fields <= 0) { set_error("lb_odometry_submit: null argument"); return LB_ERR_INVALID_ARG; }
+  return submit_job(h, "lb_odometry_submit", n_pts, point_step, fields, n_fields, mem, guess, filtered_out, mem_filtered,
+                    ticket, [&](Job& j) { j.scan = scan; });
+}
+
+int lb_odometry_submit_merged(lb_odometry* h, const lb_voxel_input* inputs, int n_inputs, uint32_t point_step,
+                              const lb_field* fields, int n_fields, int mem, const float* guess, uint8_t* filtered_out,
+                              int mem_filtered, uint64_t* ticket) {
+  if (!h || !inputs || !fields || n_fields <= 0) { set_error("lb_odometry_submit_merged: null argument"); return LB_ERR_INVALID_ARG; }
+  if (n_inputs < 1 || n_inputs > MAX_LIDARS) {
+    set_error("lb_odometry_submit_merged: 1 to %d input clouds, got %d", MAX_LIDARS, n_inputs);
+    return LB_ERR_INVALID_ARG;
+  }
+  size_t n_pts = 0;
+  for (int i = 0; i < n_inputs; i++) {
+    if (inputs[i].n_pts && !inputs[i].data) { set_error("lb_odometry_submit_merged: null input cloud %d", i); return LB_ERR_INVALID_ARG; }
+    n_pts += inputs[i].n_pts;
+  }
+  return submit_job(h, "lb_odometry_submit_merged", n_pts, point_step, fields, n_fields, mem, guess, filtered_out,
+                    mem_filtered, ticket, [&](Job& j) {
+                      j.n_inputs = n_inputs;
+                      for (int i = 0; i < n_inputs; i++) {
+                        j.in_data[i] = inputs[i].data; j.in_pts[i] = inputs[i].n_pts;
+                        j.has_T[i] = inputs[i].transform != nullptr;     // copied: the caller's array may go now
+                        if (j.has_T[i]) memcpy(j.T[i], inputs[i].transform, sizeof(j.T[i]));
+                      }
+                    });
 }
 
 int lb_odometry_next(lb_odometry* h, lb_odometry_result* r, int block) {
@@ -829,6 +899,13 @@ int lb_locus_submit(lb_locus* c, const uint8_t* scan, size_t n_pts, uint32_t poi
                     int n_fields, int mem, const float* guess, uint8_t* filtered_out, int mem_filtered, uint64_t* ticket) {
   if (!c) { set_error("lb_locus_submit: null handle"); return LB_ERR_INVALID_ARG; }
   return lb_odometry_submit(c->core, scan, n_pts, point_step, fields, n_fields, mem, guess, filtered_out, mem_filtered, ticket);
+}
+
+int lb_locus_submit_merged(lb_locus* c, const lb_voxel_input* inputs, int n_inputs, uint32_t point_step, const lb_field* fields,
+                           int n_fields, int mem, const float* guess, uint8_t* filtered_out, int mem_filtered, uint64_t* ticket) {
+  if (!c) { set_error("lb_locus_submit_merged: null handle"); return LB_ERR_INVALID_ARG; }
+  return lb_odometry_submit_merged(c->core, inputs, n_inputs, point_step, fields, n_fields, mem, guess, filtered_out,
+                                   mem_filtered, ticket);
 }
 
 int lb_locus_next(lb_locus* c, lb_locus_result* r, int block) {

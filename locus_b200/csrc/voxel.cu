@@ -570,6 +570,21 @@ static int voxel_create_impl(int device, void* stream, bool ext, lb_voxel** out)
   return LB_OK;
 }
 
+namespace lb {
+// Size the filter's scratch for raw scans of up to n_pts points of up to max_step bytes (host staging, keys, records,
+// look-back words, sort buffers), so that no later call on such scans allocates.  The lidar pipelines call it at
+// creation: their raw scan can grow mid-stream (a lidar comes back), and a cudaMalloc there would synchronise the
+// whole device.  Results do not depend on the capacities.
+int voxel_reserve(lb_voxel* h, size_t n_pts, uint32_t max_step) {
+  if (!h || n_pts == 0 || n_pts > 0x7ffffff0ull) { set_error("voxel_reserve: bad argument"); return LB_ERR_INVALID_ARG; }
+  LB_CUDA(cudaSetDevice(h->c.device));
+  LB_TRY(h->d_in.ensure(n_pts * max_step));
+  LB_TRY(h->keys.ensure(n_pts)); LB_TRY(h->seg_status.ensure((size_t)cdiv((long long)n_pts, VG_SEG_TILE)));
+  LB_TRY(h->rec.ensure(n_pts));
+  return radix_sort_reserve(h->c, h->sort, n_pts);
+}
+}  // namespace lb
+
 extern "C" {
 
 int lb_voxel_create(int device, lb_voxel** h) { return voxel_create_impl(device, nullptr, false, h); }

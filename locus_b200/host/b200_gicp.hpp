@@ -301,6 +301,13 @@ class B200Odometry {
     return lb_odometry_submit(h_, scan, n_pts, point_step, fields.data(), (int)fields.size(), LB_MEM_HOST,
                               prior ? prior->data() : nullptr, filtered_out, LB_MEM_HOST, ticket) == LB_OK;
   }
+  // one scan of 1..3 lidars merged in the VoxelGrid stage, in the merger's alive_keys_ order (lb_odometry_submit_merged:
+  // each input's transform is copied here, its points must stay valid until the result is returned)
+  bool submitMerged(const std::vector<lb_voxel_input>& inputs, uint32_t point_step, const std::vector<lb_field>& fields,
+                    const Matrix4f* prior = nullptr, uint8_t* filtered_out = nullptr, uint64_t* ticket = nullptr) {
+    return lb_odometry_submit_merged(h_, inputs.data(), (int)inputs.size(), point_step, fields.data(), (int)fields.size(),
+                                     LB_MEM_HOST, prior ? prior->data() : nullptr, filtered_out, LB_MEM_HOST, ticket) == LB_OK;
+  }
   // false when nothing is ready (block == false) or nothing is pending
   bool next(lb_odometry_result* r, bool block = true) { return lb_odometry_next(h_, r, block ? 1 : 0) == LB_OK; }
   size_t pending() const { size_t n = 0; lb_odometry_pending(h_, &n); return n; }
@@ -336,6 +343,12 @@ class B200Locus {
               const Matrix4f* prior = nullptr, uint8_t* filtered_out = nullptr, uint64_t* ticket = nullptr) {
     return lb_locus_submit(h_, scan, n_pts, point_step, fields.data(), (int)fields.size(), LB_MEM_HOST,
                            prior ? prior->data() : nullptr, filtered_out, LB_MEM_HOST, ticket) == LB_OK;
+  }
+  // as B200Odometry::submitMerged (lb_locus_submit_merged); the keyframe the map receives is the merged filtered scan
+  bool submitMerged(const std::vector<lb_voxel_input>& inputs, uint32_t point_step, const std::vector<lb_field>& fields,
+                    const Matrix4f* prior = nullptr, uint8_t* filtered_out = nullptr, uint64_t* ticket = nullptr) {
+    return lb_locus_submit_merged(h_, inputs.data(), (int)inputs.size(), point_step, fields.data(), (int)fields.size(),
+                                  LB_MEM_HOST, prior ? prior->data() : nullptr, filtered_out, LB_MEM_HOST, ticket) == LB_OK;
   }
   bool next(lb_locus_result* r, bool block = true) { return lb_locus_next(h_, r, block ? 1 : 0) == LB_OK; }
   size_t pending() const { size_t n = 0; lb_locus_pending(h_, &n); return n; }

@@ -2,6 +2,7 @@
 // that reads like PointCloudOdometry::UpdateICP (PointCloudOdometry.cc:249-269).
 // Built by __graft_entry__.build(); needs a GPU to run.
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <vector>
 
@@ -108,6 +109,27 @@ int main() {
     lb_locus_result l0, l1;
     if (rc == 0 && (!loc.next(&l0) || !loc.next(&l1) || !l0.keyframe || !l1.has_localization || l1.status != LB_OK)) rc = 13;
     if (rc == 0) std::printf("locus: L t=(%.4f %.4f), map %zu points\n", l1.pose[3], l1.pose[7], l1.map_size);
+  }
+  // a robot with three lidars: one scan whose three clouds (x, y, z, intensity records) are merged, moved into
+  // base_link and filtered in the VoxelGrid stage, in the merger's order; the first scan seeds the map
+  if (rc == 0 && lb_submap_clear(map) != LB_OK) rc = 14;
+  if (rc == 0) {
+    std::vector<lb_field> xyzi(fields);
+    xyzi.push_back(lb_field{});
+    std::snprintf(xyzi[3].name, sizeof(xyzi[3].name), "intensity");
+    xyzi[3].offset = offsetof(PointF, intensity); xyzi[3].datatype = LB_FLOAT32; xyzi[3].count = 1;
+    B200Locus loc(0, 1, 3 * reference.size(), sizeof(PointF), map);
+    loc.setLeafSize(0.05f);
+    if (!loc.applyParams()) rc = 15;
+    const Matrix4f mounts[3] = {{1, 0, 0, 0.3f, 0, 1, 0, 0, 0, 0, 1, 0.4f, 0, 0, 0, 1},
+                                {-1, 0, 0, -0.2f, 0, -1, 0, 0.25f, 0, 0, 1, 0.3f, 0, 0, 0, 1},
+                                {0, -1, 0, -0.2f, 1, 0, 0, -0.25f, 0, 0, 1, 0.3f, 0, 0, 0, 1}};
+    std::vector<lb_voxel_input> lidars(3);
+    for (int i = 0; i < 3; i++)
+      lidars[(size_t)i] = lb_voxel_input{reinterpret_cast<const uint8_t*>(reference.data()), reference.size(), mounts[i].data()};
+    lb_locus_result m0;
+    if (rc == 0 && (!loc.submitMerged(lidars, sizeof(PointF), xyzi) || !loc.next(&m0) || m0.status != LB_OK || !m0.keyframe)) rc = 16;
+    if (rc == 0) std::printf("locus, three lidars: %zu filtered points, map %zu points\n", m0.n_filtered, m0.map_size);
   }
   lb_submap_destroy(map);
   return rc;

@@ -27,6 +27,15 @@ alternated --reps times (default here 3).  Stage L bounds the chain, so its busy
 the line reports scans/s and stage L busy ms per scan for both arms, and how many timed scans kept bit-equal poses.
 
   python tools/bench_locus.py --icp-covariance --scans 60 --depth 3 --reps 3
+
+With --lidars 3 every scan is the three lidars of gen_lidar.LIDAR_MOUNTS (tools/gen_lidar.merged_stream, ~390 k raw
+points at 64 x 2048), sensor frame, merged in the VoxelGrid stage with their sensor -> base_link transforms, PassThrough
+and BodyFilter on.  The arms are those of the default run: seq_* calls lb_voxel_filter_merged and then the blocking
+chain, chain_* submits each scan with lb_locus_submit_merged (scans on the host: the pageable host-to-device copy of
+the three clouds is part of stage V).  The line adds stage V busy ms per scan of the chain arms.  --leaf sets the
+VoxelGrid leaf (default here 0.5, which keeps the filtered scans within the SM budget of DESIGN.md 4i).
+
+  python tools/bench_locus.py --lidars 3 --scans 60 --depth 3 --reps 3
 """
 import argparse
 import ctypes as C
@@ -197,6 +206,147 @@ def pipelined(lb, blobs, d_blobs, prefill, params, device, depth, prefill_n=None
     return dt, res, times
 
 
+def merged_inputs(scans, mounts):
+    return [[(b, M) for b, M in zip(sc, mounts)] for sc in scans]
+
+
+def sequential_merged(lb, scans, d_scans, mounts, prefill, params, device, leaf, setup):
+    """--lidars: the chain as blocking calls, the lidars merged by lb_voxel_filter_merged (host or device clouds)"""
+    import torch
+    P = lb.locus_params(**params)
+    vg = lb.VoxelGridB200(); setup(vg, leaf)
+    odo, loc = lb.GicpB200(), lb.GicpB200()
+    C.memmove(C.byref(odo._p), C.byref(P.odometry), C.sizeof(P.odometry)); odo._apply()
+    C.memmove(C.byref(loc._p), C.byref(P.localization), C.sizeof(P.localization)); loc._apply()
+    m = lb.SubmapB200(0, MAP_RES)
+    m.InsertPoints(prefill)
+    n = max(sum(b.size for b in sc) for sc in scans) // STEP
+    d_f = [torch.empty(n * STEP, dtype=torch.uint8, device="cuda") for _ in range(2)]
+    chain = LO.LocusChain(P)
+    fields = lb.api.VoxelGridB200._fields(lb.xyzi_fields())
+    Ts = [np.ascontiguousarray(M, np.float32).reshape(16) for M in mounts]
+    recs = []
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    prev = None
+    for k in range(len(scans)):
+        if device:
+            arr = (lb.api.VoxelInput * len(scans[k]))()
+            for i, d in enumerate(d_scans[k]):
+                arr[i].data = d.data_ptr(); arr[i].n_pts = d.numel() // STEP; arr[i].transform = Ts[i].ctypes.data_as(C.c_void_p).value
+            cur = d_f[k % 2]
+            nf = C.c_size_t(0)
+            lb.api._check(lb.lib().lb_voxel_filter_merged(vg._h, arr, len(scans[k]), STEP, fields, len(fields), C.c_void_p(cur.data_ptr()),
+                                                          n, C.byref(nf), None, lb.LB_MEM_DEVICE, lb.LB_MEM_DEVICE))
+            src = (cur.data_ptr(), nf.value, STEP)
+        else:
+            f = vg.filterMerged(scans[k], STEP, lb.xyzi_fields(), mounts)
+            src = (np.ascontiguousarray(f).view(np.float32).reshape(-1, 8)[:, :3].copy(), None, None)
+        odoT = None
+        if prev is not None:
+            odo.setInputSource(*src); odo.setInputTarget(*prev)
+            odo.align()
+            odoT = odo.getFinalTransformation()
+        loc.setInputSource(*src)
+        out = {}
+
+        def localize(Gs):
+            loc.setTargetSubmap(m)
+            out["loc"] = loc.align(Gs)
+            return loc.getFinalTransformation()
+
+        rec = chain.scan(True, odoT, localize, lambda T: m.InsertPoints(loc.transformSource(T)), lambda c, half: m.Refresh(c, half))
+        rec["loc_T"] = np.array(out["loc"].final_transformation, np.float32) if "loc" in out else None
+        recs.append(rec)
+        prev = src
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    m.close()
+    return dt, recs
+
+
+def pipelined_merged(lb, scans, d_scans, mounts, prefill, params, device, depth, leaf, setup):
+    m = lb.SubmapB200(0, MAP_RES)
+    m.InsertPoints(prefill)
+    n = max(sum(b.size for b in sc) for sc in scans) // STEP
+    ch = lb.LocusB200(m, 0, depth=depth, max_points=n, max_point_step=STEP, **params)
+    setup(ch.voxel, leaf)
+    fields = lb.api.VoxelGridB200._fields(lb.xyzi_fields())
+    res = []
+    t0 = time.perf_counter()
+    for k in range(len(scans)):
+        if device:
+            ch.submit_merged([(d.data_ptr(), d.numel() // STEP) for d in d_scans[k]], STEP, fields, mounts, mem=lb.LB_MEM_DEVICE)
+        else:
+            ch.submit_merged(scans[k], STEP, fields, mounts)
+        r = ch.next(block=False)
+        while r is not None:
+            res.append(r)
+            r = ch.next(block=False)
+    while len(res) < len(scans):
+        res.append(ch.next())
+    dt = time.perf_counter() - t0
+    times = ch.stageTimes()
+    ch.close()
+    m.close()
+    return dt, res, times
+
+
+def lidars(lb, a, line):
+    """--lidars 3: three lidars per scan merged in stage V; blocking calls against the pipeline, host and device clouds"""
+    import torch
+    scene, poses, scans, mounts = G.merged_stream(a.seed, a.scans, a.beams, a.az)
+    body = ([-0.6, -0.45, -0.5], [0.6, 0.45, 1.0])
+
+    def setup(v, leaf):
+        v.setLeafSize(leaf); v.setFilterFieldName("z"); v.setFilterLimits(-100.0, 100.0)
+        v.setInputPassThrough("z", -100.0, 100.0)
+        v.setBodyFilter(body[0], body[1], 0.0)
+
+    world = G.world_points(scene, [poses[0], G.pose_matrix([1.0, 0.5, 0.0], [0, 0, 0.3])], a.seed, a.beams, a.az)
+    vg = lb.VoxelGridB200(); vg.setLeafSize(0.2)
+    prefill = np.ascontiguousarray(vg.filter(G.xyz_blob(world), STEP, lb.xyzi_fields())).view(np.float32).reshape(-1, 8)[:, :3].copy()
+    params = dict(translation_threshold_kf=0.6, refresh_every=2)
+    leaf = a.leaf if a.leaf else 0.5
+    line.update(raw_points_per_scan=int(np.mean([sum(b.size for b in sc) // STEP for sc in scans])), lidars=3,
+                params=dict(params, leaf=leaf, map_resolution=MAP_RES, passthrough_z=[-100.0, 100.0], body_filter=body))
+    d_scans = [[torch.from_numpy(b).cuda() for b in sc] for sc in scans]
+    arms = ("seq_host", "chain_host", "seq_device", "chain_device")
+
+    def run(arm):
+        dev = arm.endswith("device")
+        if arm.startswith("seq"):
+            return sequential_merged(lb, scans, d_scans, mounts, prefill, params, dev, leaf, setup)
+        return pipelined_merged(lb, scans, d_scans, mounts, prefill, params, dev, a.depth, leaf, setup)
+
+    ref = None
+    for arm in arms:                     # one untimed pass each: modules, allocations
+        out = run(arm)
+        if arm == "seq_host":
+            ref = out[1]
+    for rep in range(a.reps):
+        for arm in arms:
+            out = run(arm)
+            dt = out[0]
+            entry = dict(scans_per_s=a.scans / dt, ms_per_scan=1e3 * dt / a.scans)
+            if arm.startswith("seq"):
+                entry["pose_mismatches_vs_seq_host"] = sum(not np.array_equal(x["L"].view(np.uint64), y["L"].view(np.uint64))
+                                                           for x, y in zip(out[1], ref))
+            else:
+                res, times = out[1], out[2]
+                entry.update(bit_equal_scans_vs_seq_host=len(res) - same(res, ref), stage_times=times,
+                             stage_v_busy_ms_per_scan=1e3 * times["voxel_busy_s"] / max(times["filtered"], 1),
+                             filtered_points_mean=float(np.mean([r.n_filtered for r in res])),
+                             filtered_points_max=int(max(r.n_filtered for r in res)),
+                             keyframes=sum(r.keyframe for r in res), crops=sum(1 for r in res if r.n_removed))
+            line["arms"].setdefault(arm, []).append(entry)
+    for arm in arms:
+        line["best_scans_per_s_" + arm] = max(x["scans_per_s"] for x in line["arms"][arm])
+    for dev in ("host", "device"):
+        line["median_stage_v_busy_ms_chain_" + dev] = float(np.median([x["stage_v_busy_ms_per_scan"] for x in line["arms"]["chain_" + dev]]))
+        line["speedup_" + dev] = line["best_scans_per_s_chain_" + dev] / line["best_scans_per_s_seq_" + dev]
+
+
 def same(res, recs):
     bad = 0
     for r, e in zip(res, recs):
@@ -293,12 +443,20 @@ def main():
     ap.add_argument("--front-end", action="store_true", help="compare the current chain with LOCUS's shipped front end")
     ap.add_argument("--icp-covariance", action="store_true",
                     help="the shipped chain with and without the localization's ICP covariance (--reps defaults to 3)")
+    ap.add_argument("--lidars", type=int, default=1, choices=(1, 3),
+                    help="3: every scan is three lidars merged in the VoxelGrid stage (lb_locus_submit_merged)")
+    ap.add_argument("--leaf", type=float, default=None, help="VoxelGrid leaf of --lidars 3 (default 0.5)")
     a = ap.parse_args()
     if a.icp_covariance and "--reps" not in sys.argv:
         a.reps = 3
     import torch
     import locus_b200 as lb
     assert lb.device_count() > 0, "bench_locus needs a CUDA device"
+    if a.lidars == 3:
+        line = {"scans": a.scans, "depth": a.depth, "card": card(), "arms": {}}
+        lidars(lb, a, line)
+        emit(line, a.out)
+        return
     scene, poses, blobs = G.stream(a.seed, a.scans, a.beams, a.az)
     world = G.world_points(scene, [poses[0], G.pose_matrix([1.0, 0.5, 0.0], [0, 0, 0.3])], a.seed, a.beams, a.az)
     vg = lb.VoxelGridB200(); vg.setLeafSize(0.2)

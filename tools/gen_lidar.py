@@ -202,6 +202,22 @@ def merged_scan(seed, beams=64, az=2048):
     return world_points(make_scene(seed), LIDAR_MOUNTS, seed, beams, az)
 
 
+def _merged_job(a):
+    scene, P, seed, beams, az = a
+    return [scan(scene, P @ M, seed * 3 + i, beams, az) for i, M in enumerate(LIDAR_MOUNTS)]
+
+
+def merged_stream(seed, n_scans, beams=64, az=2048):
+    """A robot with the three lidars of LIDAR_MOUNTS driving the trajectory of stream(seed, n_scans): per scan k the
+    three SENSOR-frame blobs of the mounts at base pose P_k (scan(scene, P_k @ M_i, ...)), in merger order.  Returns
+    (scene, base poses P_k (the ground truth), [[blob_a, blob_b, blob_c] per scan], mounts as float32 4x4 sensor ->
+    base_link)."""
+    scene = make_scene(seed)
+    poses = trajectory(seed, n_scans)
+    scans = _map_jobs(_merged_job, [(scene, poses[k], seed * 7919 + k, beams, az) for k in range(n_scans)])
+    return scene, poses, scans, [M.astype(np.float32) for M in LIDAR_MOUNTS]
+
+
 def perturbed_prior(T, seed, t=0.05, r_deg=0.4):
     """the odometry estimate handed to scan-to-submap registration as its guess: the true pose off by a few
     centimetres / tenths of a degree (PointCloudLocalization.cc:181-200 pre-transforms the query with it)"""
