@@ -43,7 +43,7 @@ struct Cloud {
   size_t ncells = 0;
   uint64_t generation = 0;
   bool index_dirty = false;    // uploaded + geometry chosen, CSR index not built yet (built lazily in align)
-  int keys_slot = -1;          // >= 0: that slot's scratch holds this cloud's cell keys and per-cell counts for `geom`
+  int keys_slot = -1;          // >= 0: that slot's scratch holds this cloud's cell keys, occupancy marks and sort histograms for `geom`
                                // (left there by the accepted round of the occupancy probe)
   uint64_t dense_generation = 0;   // generation for which dense_fraction was measured (lb_gicp_nn_target picks its kernel by it)
   double dense_fraction = 0.0;     // share of the points that sit in cells with more than 32 points
@@ -78,14 +78,26 @@ struct Scratch {
   DBuf<uint32_t> keys, cell_cnt, worklist;   // worklist: queries the quad k-NN kernel hands to the tail kernel
   SortWork sort;
   ScanWork scan;
-  BBoxAcc* d_acc = nullptr; BBoxAcc* h_acc = nullptr;
+  IndexState* d_st = nullptr; IndexState* h_st = nullptr;   // state of the index build and its pinned host copy
   uint32_t* d_u32 = nullptr; uint32_t* h_u32 = nullptr;
+  bool marks_zero = false;       // every word of cell_cnt (the occupancy marks) is zero
+  bool wl_zero = false;          // d_st->wl is zero
+  // the occupancy marks for a grid of `cells` cells, all zero (a probe round that was accepted is cleared by
+  // grid_reorder_kernel; anything else -- a rejected round, a grown buffer -- costs a memset here)
+  int ensure_marks(size_t cells) {
+    const size_t cap = cell_cnt.cap;
+    LB_TRY(cell_cnt.ensure(cells));
+    if (cell_cnt.cap != cap) marks_zero = false;
+    if (!marks_zero && cell_cnt.cap) LB_CUDA(cudaMemsetAsync(cell_cnt.p, 0, cell_cnt.cap * sizeof(uint32_t), c.stream));
+    marks_zero = true;
+    return LB_OK;
+  }
   void release() {
     stage.release(); keys.release(); cell_cnt.release(); worklist.release();
     sort.ka.release(); sort.kb.release(); sort.va.release(); sort.vb.release(); sort.state.release();
     scan.sums.release();
-    if (d_acc) cudaFree(d_acc);
-    if (h_acc) cudaFreeHost(h_acc);
+    if (d_st) cudaFree(d_st);
+    if (h_st) cudaFreeHost(h_st);
     if (d_u32) cudaFree(d_u32);
     if (h_u32) cudaFreeHost(h_u32);
   }
@@ -275,8 +287,9 @@ int gicp_create_impl(int device, void* stream, bool ext, lb_gicp** out) {
     Scratch& S = h->sc[k];
     S.c = h->c; S.c.own_stream = false; S.c.launches = 0;
     if (k == 1) S.c.stream = h->stream2;
-    ok = cudaMalloc((void**)&S.d_acc, sizeof(BBoxAcc)) == cudaSuccess &&
-         cudaMallocHost((void**)&S.h_acc, sizeof(BBoxAcc)) == cudaSuccess &&
+    ok = cudaMalloc((void**)&S.d_st, sizeof(IndexState)) == cudaSuccess &&
+         cudaMemset(S.d_st, 0, sizeof(IndexState)) == cudaSuccess &&
+         cudaMallocHost((void**)&S.h_st, sizeof(IndexState)) == cudaSuccess &&
          cudaMalloc((void**)&S.d_u32, 8 * sizeof(uint32_t)) == cudaSuccess &&
          cudaMallocHost((void**)&S.h_u32, 8 * sizeof(uint32_t)) == cudaSuccess;
   }
@@ -292,7 +305,7 @@ int gicp_create_impl(int device, void* stream, bool ext, lb_gicp** out) {
   for (int i = 0; ok && i < 4; i++) ok = cudaEventCreate(&h->ev[i]) == cudaSuccess;
   if (ok) ok = cudaMemset(h->d_barrier, 0, 2 * sizeof(unsigned)) == cudaSuccess;
   if (ok) {
-    for (int k = 0; k < 2; k++) bbox_init_kernel<<<1, 32, 0, h->c.stream>>>(h->sc[k].d_acc);
+    for (int k = 0; k < 2; k++) bbox_init_kernel<<<1, 32, 0, h->c.stream>>>(&h->sc[k].d_st->acc);
     ok = cudaStreamSynchronize(h->c.stream) == cudaSuccess;
   }
   if (!ok) {
@@ -451,80 +464,68 @@ int upload_cloud(lb_gicp* h, Cloud& cl, int slot, const void* pts, size_t n, siz
   LB_TRY(cl.raw.ensure(maxn)); LB_TRY(cl.pts.ensure(maxn));
   if (normal_off >= 0) LB_TRY(cl.nrm.ensure(maxn));
   if (same_as && !(same_as->valid && same_as->n == n && same_as->has_normals == (normal_off >= 0))) same_as = nullptr;
-  if (same_as) LB_CUDA(cudaMemsetAsync(S.d_u32 + 2, 0, sizeof(uint32_t), c.stream));
+  const bool auto_cell = !(h->P.index_cell_size > 0.f);
+  if (auto_cell) {
+    LB_TRY(S.keys.ensure(n));
+    LB_TRY(radix_sort_reserve(c, S.sort, n));
+    LB_TRY(S.ensure_marks(0));
+  }
   gather_cloud_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(d_src, N, (uint32_t)stride, (uint32_t)xyz_off, (int)normal_off,
-                                                          cl.raw.p, normal_off >= 0 ? cl.nrm.p : nullptr, S.d_acc,
+                                                          cl.raw.p, normal_off >= 0 ? cl.nrm.p : nullptr, S.d_st,
                                                           same_as ? same_as->raw.p : nullptr,
-                                                          same_as && normal_off >= 0 ? same_as->nrm.p : nullptr, S.d_u32 + 2);
+                                                          same_as && normal_off >= 0 ? same_as->nrm.p : nullptr);
   c.launches += 1;
-  LB_CUDA(cudaMemcpyAsync(S.h_acc, S.d_acc, sizeof(BBoxAcc), cudaMemcpyDeviceToHost, c.stream));
-  if (same_as) LB_CUDA(cudaMemcpyAsync(S.h_u32 + 2, S.d_u32 + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
-  bbox_init_kernel<<<1, 32, 0, c.stream>>>(S.d_acc);   // accumulator clean for the next upload
-  c.launches += 1;
+  // Automatic cell size: the first occupancy-probe round follows at once, on the grid the gather's last CTA chose.
+  // The cell size is a pure function of the cloud (no memory of earlier clouds): the same cloud gives the same
+  // grid, hence the same summation order in the align kernel and bit-identical poses, whichever handle or
+  // pipeline worker sees it.  The accepted round's keys and sort histograms are what finish_index needs.
+  if (auto_cell && S.cell_cnt.cap) {
+    grid_index_keys_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(cl.raw.p, N, GridGeom(), true, S.d_st, S.keys.p, S.cell_cnt.p, S.cell_cnt.cap,
+                                                               S.sort.dev(), S.sort.status(), rs_tiles(n));
+    c.launches += 1;
+    S.marks_zero = false;
+  }
+  // the one round trip of an upload: bounding box, finite count, "same cloud" flag, the device's grid and its occupancy
+  LB_CUDA(cudaMemcpyAsync(S.h_st, S.d_st, sizeof(IndexState), cudaMemcpyDeviceToHost, c.stream));
   LB_CUDA(cudaStreamSynchronize(c.stream));
-  if (S.h_acc->count != N) {
-    set_error("%s: cloud holds %u non-finite points; GICP inputs must be dense (PCL kd-tree precondition)", what, N - S.h_acc->count);
+  const IndexState& st = *S.h_st;
+  if (auto_cell && S.cell_cnt.cap && !st.probed) S.marks_zero = true;     // the key kernel stood aside: nothing was marked
+  if (st.count != N) {
+    set_error("%s: cloud holds %u non-finite points; GICP inputs must be dense (PCL kd-tree precondition)", what, N - st.count);
     return LB_ERR_INVALID_ARG;
   }
-  if (same_as && S.h_u32[2] == 0) return LB_SAME_CLOUD;
+  if (same_as && st.differs == 0) return LB_SAME_CLOUD;
   float mn[3], mx[3];
-  for (int d = 0; d < 3; d++) { mn[d] = ord2f(S.h_acc->mn[d]); mx[d] = ord2f(S.h_acc->mx[d]); }
-  float ext[3] = {mx[0] - mn[0], mx[1] - mn[1], mx[2] - mn[2]};
-
-  auto make_geom = [&](float cell) {
-    GridGeom g;
-    const int MAXDIM = 16384;
-    const double MAXCELLS = 64.0 * 1024 * 1024;
-    for (;;) {
-      g.ox = mn[0]; g.oy = mn[1]; g.oz = mn[2];
-      g.h = cell; g.inv_h = 1.0f / cell;
-      double fx = floor((double)(ext[0] * g.inv_h)) + 1, fy = floor((double)(ext[1] * g.inv_h)) + 1, fz = floor((double)(ext[2] * g.inv_h)) + 1;
-      if (fx <= MAXDIM && fy <= MAXDIM && fz <= MAXDIM && fx * fy * fz <= MAXCELLS) {
-        g.nx = (int)fx; g.ny = (int)fy; g.nz = (int)fz;
-        return g;
-      }
-      cell *= 1.5f;
-    }
-  };
+  for (int d = 0; d < 3; d++) { mn[d] = ord2f(st.mn[d]); mx[d] = ord2f(st.mx[d]); }
+  const float ext[3] = {mx[0] - mn[0], mx[1] - mn[1], mx[2] - mn[2]};
 
   GridGeom g;
-  float cell = h->P.index_cell_size;
-  if (cell > 0.f) {
-    g = make_geom(cell);
+  if (!auto_cell) {
+    g = grid_make_geom(mn, ext, h->P.index_cell_size);
   } else {
-    // automatic: aim at ~6 points per occupied cell (h ~ 2.5 x point spacing on a surface, so the
-    // 20-NN radius is about one cell and a 1-NN probe rarely leaves the 3x3x3 block)
-    double area = 2.0 * ((double)ext[0] * ext[1] + (double)ext[1] * ext[2] + (double)ext[0] * ext[2]);
-    double diag = sqrt((double)ext[0] * ext[0] + (double)ext[1] * ext[1] + (double)ext[2] * ext[2]);
-    if (!(area > 0)) area = diag * diag;
-    double spacing = sqrt(area / (double)(N ? N : 1));
-    cell = (float)(1.3 * spacing);     // first guess; lidar scans concentrate their points, so the bbox-surface spacing
-                                       // overestimates: 1.3x lands inside the accepted occupancy band in one round
-    if (!(cell > 0.f)) cell = 1.0f;
-    const double target = 6.0;
-    // The cell size is a pure function of the cloud (no memory of earlier clouds): the same cloud gives the same
-    // grid, hence the same summation order in the align kernel and bit-identical poses, whichever handle or
-    // pipeline worker sees it.  The accepted round's keys and per-cell counts are what finish_index needs.
-    LB_TRY(S.keys.ensure(n));
-    for (int round = 0; round < 4; round++) {
-      g = make_geom(cell);
-      size_t nc = (size_t)g.nx * g.ny * g.nz;
-      LB_TRY(S.cell_cnt.ensure(nc + 1));
-      LB_CUDA(cudaMemsetAsync(S.cell_cnt.p, 0, (nc + 1) * sizeof(uint32_t), c.stream));
-      LB_CUDA(cudaMemsetAsync(S.d_u32, 0, sizeof(uint32_t), c.stream));
-      grid_keys_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(cl.raw.p, N, g, S.keys.p, nullptr);
-      grid_occupancy_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(S.keys.p, N, S.cell_cnt.p, S.d_u32);
-      c.launches += 2;
-      LB_CUDA(cudaMemcpyAsync(S.h_u32, S.d_u32, sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+    float cell = grid_auto_cell(ext, N);
+    g = grid_make_geom(mn, ext, cell);
+    int round = 0;
+    bool accepted = false;
+    // the device's round counts when it ran on exactly this grid; otherwise (no room for the marks yet, on a handle's
+    // first clouds) the rounds below start from the beginning
+    if (st.probed && !memcmp(&g, &st.geom, sizeof(GridGeom))) {
+      h->probe_rounds++;
+      accepted = grid_probe_accept(N, st.n_occ, g.h, &cell);
+      round = 1;
+    }
+    for (; !accepted && round < GRID_PROBE_ROUNDS; round++) {
+      g = grid_make_geom(mn, ext, cell);
+      LB_TRY(S.ensure_marks((size_t)g.nx * g.ny * g.nz + 1));
+      LB_CUDA(cudaMemsetAsync(&S.d_st->n_occ, 0, sizeof(uint32_t), c.stream));
+      grid_index_keys_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(cl.raw.p, N, g, false, S.d_st, S.keys.p, S.cell_cnt.p, S.cell_cnt.cap,
+                                                                 S.sort.dev(), S.sort.status(), rs_tiles(n));
+      c.launches += 1;
+      S.marks_zero = false;
+      LB_CUDA(cudaMemcpyAsync(&S.h_st->n_occ, &S.d_st->n_occ, sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
       LB_CUDA(cudaStreamSynchronize(c.stream));
       h->probe_rounds++;
-      double occ = (double)N / (double)(S.h_u32[0] ? S.h_u32[0] : 1);
-      if (occ >= target / 2 && occ <= target * 2) break;
-      if (N <= 8 || S.h_u32[0] <= 1) break;
-      double scale = sqrt(target / occ);
-      if (scale > 4) scale = 4;
-      if (scale < 0.25) scale = 0.25;
-      cell = g.h * (float)scale;
+      accepted = grid_probe_accept(N, st.n_occ, g.h, &cell);
     }
     cl.keys_slot = slot;
   }
@@ -581,25 +582,26 @@ int finish_index(lb_gicp* h, Cloud& cl, int slot) {
   Scratch& S = h->sc[slot];
   Ctx& c = S.c;
   const uint32_t N = (uint32_t)cl.n;
-  int key_bits = 1;
-  while (key_bits < 32 && (1ull << key_bits) < (uint64_t)cl.ncells) key_bits++;
-  const bool have_keys = cl.keys_slot == slot;     // the occupancy probe left keys + per-cell counts in this slot
+  const int key_bits = grid_key_bits(cl.ncells);
+  const bool have_keys = cl.keys_slot == slot;     // the occupancy probe left keys, marks and the sort histograms in this slot
   cl.keys_slot = -1;
   size_t& maxc = h->max_cells_seen[slot];
   if (cl.ncells + 1 > maxc) maxc = cl.ncells + 1;
   LB_TRY(cl.cell_start.ensure(maxc));
   if (!have_keys) {
     LB_TRY(S.keys.ensure(cl.n));
-    LB_TRY(S.cell_cnt.ensure(cl.ncells + 1));
-    LB_CUDA(cudaMemsetAsync(S.cell_cnt.p, 0, (cl.ncells + 1) * sizeof(uint32_t), c.stream));
-    grid_keys_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(cl.raw.p, N, cl.geom, S.keys.p, nullptr);
+    LB_TRY(radix_sort_reserve(c, S.sort, cl.n));
+    grid_index_keys_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(cl.raw.p, N, cl.geom, false, S.d_st, S.keys.p, nullptr, 0,
+                                                               S.sort.dev(), S.sort.status(), rs_tiles(cl.n));
     c.launches++;
   }
   uint32_t *sk = nullptr, *sv = nullptr;
-  LB_TRY(radix_sort_pairs(c, S.sort, S.keys.p, nullptr, cl.n, key_bits, &sk, &sv));
-  grid_reorder_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(cl.raw.p, sk, sv, N, cl.pts.p, have_keys ? nullptr : S.cell_cnt.p);
+  LB_TRY(radix_sort_scatter(c, S.sort, S.keys.p, cl.n, key_bits, &sk, &sv));
+  grid_reorder_kernel<<<cdiv(N, 256), 256, 0, c.stream>>>(cl.raw.p, sk, sv, N, (uint32_t)cl.ncells, cl.pts.p, cl.cell_start.p,
+                                                          have_keys ? S.cell_cnt.p : nullptr, S.d_st->wl);
   c.launches++;
-  LB_TRY(exclusive_scan_u32(c, S.scan, S.cell_cnt.p, cl.cell_start.p, cl.ncells + 1, nullptr));
+  if (have_keys) S.marks_zero = true;
+  S.wl_zero = true;
   LB_CUDA(cudaGetLastError());
   cl.index_dirty = false;
   return LB_OK;
@@ -637,8 +639,9 @@ int compute_covariances(lb_gicp* h, Cloud& cl, int slot, bool recompute) {
         static const int ring_cap = [] { const char* e = getenv("LB_RING_CAP"); return e ? atoi(e) : 6; }();   // tuning aid; 6 was chosen on an earlier GPU, not re-tuned for the H100
         Scratch& S = h->sc[slot];
         LB_TRY(S.worklist.ensure(N));
-        uint32_t* d_wl = S.d_u32 + 4;      // [0] is the occupancy probe's counter
-        LB_CUDA(cudaMemsetAsync(d_wl, 0, 2 * sizeof(uint32_t), c.stream));     // [0] worklist count, [1] next query batch
+        uint32_t* d_wl = S.d_st->wl;       // [0] worklist count, [1] next query batch: left at zero by the index build
+        if (!S.wl_zero) LB_CUDA(cudaMemsetAsync(d_wl, 0, 2 * sizeof(uint32_t), c.stream));     // covariances again on an index built earlier
+        S.wl_zero = false;
         // tuning aid LB_KNN_DYN=1: a resident grid pulls 8-query batches from a counter (slower than the static
         // grid at 30 k and 500 k points, so off by default)
         static const int dyn = [] { const char* e = getenv("LB_KNN_DYN"); return e ? atoi(e) : 0; }();
@@ -906,7 +909,7 @@ int lb_gicp_reserve(lb_gicp* h, size_t max_points, int spare_clouds) {
   }
   for (int k = 0; k < 2; k++) {
     Scratch& S = h->sc[k];
-    LB_TRY(S.keys.ensure(max_points)); LB_TRY(S.cell_cnt.ensure(cells + 1)); LB_TRY(S.worklist.ensure(max_points));
+    LB_TRY(S.keys.ensure(max_points)); LB_TRY(S.ensure_marks(cells + 1)); LB_TRY(S.worklist.ensure(max_points));
     LB_TRY(S.sort.ka.ensure(max_points)); LB_TRY(S.sort.kb.ensure(max_points));
     LB_TRY(S.sort.va.ensure(max_points)); LB_TRY(S.sort.vb.ensure(max_points));
   }

@@ -1,8 +1,8 @@
 // gicp_kernels.cuh -- CUDA kernels of the GICP hot path (K2-K6 of SURVEY.md 2.3).
 //
 //   gather_cloud_kernel      strided caller cloud -> packed float4 (+ normals)
-//   grid_keys_kernel         K2: cell key per point
-//   grid_reorder_kernel      K2: cell-contiguous float4 copy + cell histogram
+//   grid_index_keys_kernel   K2: cell key per point + occupancy count + the sort's digit histograms
+//   grid_reorder_kernel      K2: cell-contiguous float4 copy + CSR cell offsets from the sorted keys
 //   knn_cov_quadreg_kernel   K3: k-NN(20) -> moments -> Jacobi -> regularised covariance (+ knn_cov_tail_kernel,
 //                            knn_cov_quad_kernel for k > 20)
 //   normal_cov_kernel        K3': covariance from normals (reference default mode)
@@ -39,10 +39,30 @@ constexpr int AL_SOLVE_THREADS = 32 + AL_ACC;
 constexpr int AL_SOLVE_POLL = 8;     // slot words one thread of the solve kernel polls at a time
 
 // ------------------------------------------------------------------ cloud upload
+// Device state of one slot's index build.  The first part is published by the kernels of an upload and read by the
+// host in ONE copy; the rest are the accumulators behind it, which every kernel leaves the way the next upload expects
+// them (bounding box reset, flags and tickets zero).
+struct IndexState {
+  uint32_t mn[3], mx[3];   // finite bounding box (ordered-uint encoding) ...
+  uint32_t count;          // ... and the number of finite points
+  uint32_t differs;        // the cloud is not the one it was compared with
+  GridGeom geom;           // grid of the first occupancy-probe round (grid_auto_geom of the box)
+  int key_bits;            // width of its cell keys
+  uint32_t probed;         // grid_index_keys_kernel ran on `geom`: keys, n_occ and the sort histograms are valid
+  uint32_t n_occ;          // occupied cells
+  uint32_t wl[2];          // compute_covariances: work-list count and next query batch (zeroed by grid_reorder_kernel)
+  BBoxAcc acc;
+  uint32_t differs_acc;
+  uint32_t ticket;         // last-CTA detection of gather_cloud_kernel
+};
+
+// The last CTA to finish (ticket) turns the bounding box into the first probe round's grid -- the same function the
+// host evaluates on the copy it reads back -- so the key kernel can follow without a host round trip.
 __global__ void __launch_bounds__(256)
 gather_cloud_kernel(const uint8_t* __restrict__ base, uint32_t n, uint32_t stride, uint32_t xyz_off, int normal_off,
-                    f4* __restrict__ raw, f4* __restrict__ nrm, BBoxAcc* __restrict__ acc,
-                    const f4* __restrict__ same_raw, const f4* __restrict__ same_nrm, uint32_t* __restrict__ differs) {
+                    f4* __restrict__ raw, f4* __restrict__ nrm, IndexState* __restrict__ st,
+                    const f4* __restrict__ same_raw, const f4* __restrict__ same_nrm) {
+  __shared__ bool last;
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   bool ok = false;
   float x = 0.f, y = 0.f, z = 0.f;
@@ -64,18 +84,39 @@ gather_cloud_kernel(const uint8_t* __restrict__ base, uint32_t n, uint32_t strid
         diff = diff || __float_as_uint(o.x) != __float_as_uint(m[0]) || __float_as_uint(o.y) != __float_as_uint(m[1]) || __float_as_uint(o.z) != __float_as_uint(m[2]);
       }
     }
-    if (diff) *differs = 1u;
+    if (diff) st->differs_acc = 1u;
     ok = isfinite(x) && isfinite(y) && isfinite(z);
   }
-  bbox_warp_accumulate(ok, x, y, z, acc);   // finite-point bounding box + count (accumulator was reset by the previous build)
+  bbox_warp_accumulate(ok, x, y, z, &st->acc);   // finite-point bounding box + count (accumulator was reset by the previous build)
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(&st->ticket, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last || threadIdx.x != 0) return;
+  __threadfence();
+  const uint32_t count = atomicAdd(&st->acc.count, 0u);
+  float mn[3], mx[3];
+  for (int d = 0; d < 3; d++) {
+    st->mn[d] = atomicAdd(&st->acc.mn[d], 0u); st->mx[d] = atomicAdd(&st->acc.mx[d], 0u);
+    mn[d] = ord2f(st->mn[d]); mx[d] = ord2f(st->mx[d]);
+  }
+  const uint32_t differs = atomicAdd(&st->differs_acc, 0u);
+  st->count = count; st->differs = differs;
+  // a refused cloud (non-finite points) or one that is adopted instead (equal to `same_raw`) gets no keys
+  const bool index = count == n && !(same_raw && !differs);
+  if (index) {
+    const GridGeom g = grid_auto_geom(mn, mx, n);
+    st->geom = g;
+    st->key_bits = grid_key_bits((uint64_t)g.nx * g.ny * g.nz);
+  } else {
+    st->key_bits = 0;
+  }
+  st->probed = 0; st->n_occ = 0;
+  bbox_reset(&st->acc);            // consumed: clean for the next upload
+  st->differs_acc = 0; st->ticket = 0;
 }
 
 // ------------------------------------------------------------------ K2 index build
-struct GridGeom {
-  float ox, oy, oz, inv_h, h;
-  int nx, ny, nz;
-};
-
 __device__ __forceinline__ uint32_t cell_of(const GridGeom& g, float x, float y, float z) {
   int cx = (int)floorf((x - g.ox) * g.inv_h);
   int cy = (int)floorf((y - g.oy) * g.inv_h);
@@ -84,35 +125,86 @@ __device__ __forceinline__ uint32_t cell_of(const GridGeom& g, float x, float y,
   return (uint32_t)((cz * g.ny + cy) * g.nx + cx);
 }
 
+// Cell key per point, plus what the steps after it need, in the one pass over the points:
+//   * the digit histogram of every sort pass (rs_hist_*) and the reset of the scatters' look-back state, so the sort is
+//     its scatter passes only;
+//   * marks != nullptr (occupancy probe of the automatic cell size): first touches per cell, counted into st->n_occ.
+//     `marks` is all-zero between index builds: grid_reorder_kernel clears the words this kernel set.
+// st_geom: take the grid from the state block (the first probe round, chosen on the device by gather_cloud_kernel) and do
+// nothing when there is none or it has more cells than `marks` holds -- the host then runs the round itself.
 __global__ void __launch_bounds__(256)
-grid_keys_kernel(const f4* __restrict__ raw, uint32_t n, GridGeom g, uint32_t* __restrict__ keys, BBoxAcc* acc_to_reset) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i == 0 && acc_to_reset) bbox_reset(acc_to_reset);   // the host has consumed it: ready for the next build
-  if (i >= n) return;
-  f4 p = raw[i];
-  keys[i] = cell_of(g, p.x, p.y, p.z);
+grid_index_keys_kernel(const f4* __restrict__ raw, uint32_t n, GridGeom g, bool st_geom, IndexState* __restrict__ st,
+                       uint32_t* __restrict__ keys, uint32_t* __restrict__ marks, size_t marks_cap,
+                       RsDev* __restrict__ rs, uint32_t* __restrict__ rs_status, uint32_t rs_tiles) {
+  __shared__ uint32_t sh[RS_PASSES_MAX][256];
+  __shared__ uint32_t scan_sm[256 / 32 + 1];
+  __shared__ bool last;
+  int key_bits;
+  if (st_geom) {
+    key_bits = st->key_bits;
+    if (key_bits == 0) return;
+    g = st->geom;
+    if ((size_t)g.nx * g.ny * g.nz > marks_cap) return;
+  } else {
+    key_bits = grid_key_bits((uint64_t)g.nx * g.ny * g.nz);
+  }
+  const int passes = (key_bits + 7) >> 3;
+  for (int t = threadIdx.x; t < RS_PASSES_MAX * 256; t += 256) (&sh[0][0])[t] = 0;
+  rs_reset_lookback(rs, rs_status, rs_tiles);
+  __syncthreads();
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  uint32_t key = 0, first = 0;
+  if (i < n) {
+    const f4 p = raw[i];
+    key = cell_of(g, p.x, p.y, p.z);
+    keys[i] = key;
+    if (marks) first = (atomicAdd(&marks[key], 1u) == 0u) ? 1u : 0u;
+  }
+  if (marks) {
+    const uint32_t b = __ballot_sync(0xffffffffu, first);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(&st->n_occ, (uint32_t)__popc(b));
+    if (i == 0) st->probed = 1u;
+  }
+  rs_hist_warp_add(sh, key, i < n, passes);
+  rs_hist_flush(sh, rs, passes, scan_sm, &last);
 }
 
-// occupancy probe for the automatic cell size: marks cells, counts first touches
-__global__ void __launch_bounds__(256)
-grid_occupancy_kernel(const uint32_t* __restrict__ keys, uint32_t n, uint32_t* __restrict__ cell_cnt, uint32_t* n_occ) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  uint32_t first = 0;
-  if (i < n) first = (atomicAdd(&cell_cnt[keys[i]], 1u) == 0u) ? 1u : 0u;
-  uint32_t b = __ballot_sync(0xffffffffu, first);
-  if ((threadIdx.x & 31) == 0 && b) atomicAdd(n_occ, (uint32_t)__popc(b));
-}
-
+// Cell-contiguous copy of the points (w = original index) and the CSR offsets, read off the sorted keys: a position whose
+// key differs from its predecessor's starts its cell and the empty cells before it; the last position closes the
+// cells after its own.  The 32 lanes of a warp fill each such run of offsets together (a run of empty cells can be
+// long: whole rows and slabs of the grid of a surface-like cloud).
+// marks (nullable): the occupancy marks of the key kernel, cleared here; wl (nullable): the k-NN work-list counters.
 __global__ void __launch_bounds__(256)
 grid_reorder_kernel(const f4* __restrict__ raw, const uint32_t* __restrict__ sorted_keys,
-                    const uint32_t* __restrict__ sorted_vals, uint32_t n, f4* __restrict__ pts,
-                    uint32_t* __restrict__ cell_cnt) {
-  uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= n) return;
-  uint32_t i = sorted_vals[s];
-  f4 p = raw[i];
-  pts[s] = f4{p.x, p.y, p.z, bits_to_float((int32_t)i)};
-  if (cell_cnt) atomicAdd(&cell_cnt[sorted_keys[s]], 1u);   // null: the occupancy probe already counted
+                    const uint32_t* __restrict__ sorted_vals, uint32_t n, uint32_t ncells, f4* __restrict__ pts,
+                    uint32_t* __restrict__ cell_start, uint32_t* __restrict__ marks, uint32_t* __restrict__ wl) {
+  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s == 0 && wl) { wl[0] = 0; wl[1] = 0; }
+  uint32_t key = 0, lo = 1, hi = 0;          // this position writes cell_start[lo..hi] = s (empty when lo > hi)
+  if (s < n) {
+    const uint32_t i = sorted_vals[s];
+    const f4 p = raw[i];
+    pts[s] = f4{p.x, p.y, p.z, bits_to_float((int32_t)i)};
+    key = sorted_keys[s];
+    const uint32_t prev = s ? sorted_keys[s - 1] : 0xffffffffu;      // "cell -1" before the first position
+    if (prev != key) {
+      lo = prev + 1u; hi = key;
+      if (marks) marks[key] = 0;
+    }
+  }
+  const int lane = threadIdx.x & 31;
+  uint32_t runs = __ballot_sync(0xffffffffu, lo <= hi);
+  while (runs) {
+    const int src = __ffs(runs) - 1;
+    runs &= runs - 1;
+    const uint32_t a = __shfl_sync(0xffffffffu, lo, src), b = __shfl_sync(0xffffffffu, hi, src);
+    const uint32_t v = (s & ~31u) + (uint32_t)src;
+    for (uint64_t c = (uint64_t)a + lane; c <= b; c += 32) cell_start[c] = v;
+  }
+  if (s / 32 == (n - 1) / 32 && n > 0) {        // the warp of the last position: cells after the last key end at n
+    const uint32_t tail = __shfl_sync(0xffffffffu, key, (n - 1) & 31);
+    for (uint64_t c = (uint64_t)tail + 1 + lane; c <= ncells; c += 32) cell_start[c] = n;
+  }
 }
 
 // ------------------------------------------------------------------ K3 covariances

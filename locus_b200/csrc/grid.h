@@ -33,6 +33,78 @@ struct GridView {
   int n;                       // number of points
 };
 
+// ---- the grid a cloud gets (origin, cell size, dimensions) --------------------------------------------------------
+// One set of functions for the host driver and for the kernels of the index build, so that the geometry the device
+// chooses for a cloud and the one the host fills into GridView are the same bits.  float and double arithmetic only
+// (+, *, /, sqrt, floor: correctly rounded on both sides; the library is built without FMA contraction).  The cell size
+// decides the order of the points in memory, hence the summation order of the align and the bits of the pose.
+struct GridGeom {
+  float ox, oy, oz, inv_h, h;
+  int nx, ny, nz;
+};
+
+constexpr int GRID_MAXDIM = 16384;
+constexpr double GRID_MAXCELLS = 64.0 * 1024 * 1024;
+constexpr double GRID_TARGET_OCC = 6.0;      // points per occupied cell the automatic cell size aims at
+constexpr int GRID_PROBE_ROUNDS = 4;
+
+// Grid of cell size `cell` over the box [mn, mn + ext]; the cell grows by 1.5x until the grid fits the caps.  The loop is
+// bounded: an extent that is not finite (coordinates near FLT_MAX) can never fit and ends in a single cell.
+LB_HD GridGeom grid_make_geom(const float* mn, const float* ext, float cell) {
+  GridGeom g;
+  g.ox = mn[0]; g.oy = mn[1]; g.oz = mn[2];
+  for (int grow = 0; grow < 512; grow++) {
+    g.h = cell; g.inv_h = 1.0f / cell;
+    double fx = floor((double)(ext[0] * g.inv_h)) + 1, fy = floor((double)(ext[1] * g.inv_h)) + 1, fz = floor((double)(ext[2] * g.inv_h)) + 1;
+    if (fx <= GRID_MAXDIM && fy <= GRID_MAXDIM && fz <= GRID_MAXDIM && fx * fy * fz <= GRID_MAXCELLS) {
+      g.nx = (int)fx; g.ny = (int)fy; g.nz = (int)fz;
+      return g;
+    }
+    cell *= 1.5f;
+  }
+  g.nx = g.ny = g.nz = 1;
+  return g;
+}
+
+// First guess of the automatic cell size: aim at ~6 points per occupied cell (h ~ 2.5 x point spacing on a surface, so
+// the 20-NN radius is about one cell and a 1-NN probe rarely leaves the 3x3x3 block).  Lidar scans concentrate their
+// points, so the bbox-surface spacing overestimates: 1.3x lands inside the accepted occupancy band in one round.
+LB_HD float grid_auto_cell(const float* ext, uint32_t n) {
+  double area = 2.0 * ((double)ext[0] * ext[1] + (double)ext[1] * ext[2] + (double)ext[0] * ext[2]);
+  double diag = sqrt((double)ext[0] * ext[0] + (double)ext[1] * ext[1] + (double)ext[2] * ext[2]);
+  if (!(area > 0)) area = diag * diag;
+  double spacing = sqrt(area / (double)(n ? n : 1));
+  float cell = (float)(1.3 * spacing);
+  if (!(cell > 0.f)) cell = 1.0f;
+  return cell;
+}
+
+// The grid of the first probe round for the finite bounding box [mn, mx] of n points.
+LB_HD GridGeom grid_auto_geom(const float* mn, const float* mx, uint32_t n) {
+  const float ext[3] = {mx[0] - mn[0], mx[1] - mn[1], mx[2] - mn[2]};
+  return grid_make_geom(mn, ext, grid_auto_cell(ext, n));
+}
+
+// A probe round counted n_occ occupied cells at cell size h: true when the grid is kept (occupancy inside
+// [target / 2, 2 target], or nothing to gain from another round); otherwise *next_cell is the next round's cell size.
+LB_HD bool grid_probe_accept(uint32_t n, uint32_t n_occ, float h, float* next_cell) {
+  double occ = (double)n / (double)(n_occ ? n_occ : 1);
+  if (occ >= GRID_TARGET_OCC / 2 && occ <= GRID_TARGET_OCC * 2) return true;
+  if (n <= 8 || n_occ <= 1) return true;
+  double scale = sqrt(GRID_TARGET_OCC / occ);
+  if (scale > 4) scale = 4;
+  if (scale < 0.25) scale = 0.25;
+  *next_cell = h * (float)scale;
+  return false;
+}
+
+// width of a cell key of a grid of ncells cells
+LB_HD int grid_key_bits(uint64_t ncells) {
+  int key_bits = 1;
+  while (key_bits < 32 && (1ull << key_bits) < ncells) key_bits++;
+  return key_bits;
+}
+
 LB_HD float dist2(float ax, float ay, float az, float bx, float by, float bz) {
   float dx = ax - bx, dy = ay - by, dz = az - bz;
   float d = dx * dx;

@@ -331,6 +331,10 @@ int radix_sort_pairs(Ctx& c, SortWork& w, const uint32_t* keys_in, const uint32_
   return radix_sort_impl(c, w, keys_in, vals_in, n, key_bits, nullptr, true, keys_out, vals_out);
 }
 
+int radix_sort_scatter(Ctx& c, SortWork& w, const uint32_t* keys_in, size_t n, int key_bits, uint32_t** keys_out, uint32_t** vals_out) {
+  return radix_sort_impl(c, w, keys_in, nullptr, n, key_bits, nullptr, false, keys_out, vals_out);
+}
+
 int radix_sort_pairs_devbits(Ctx& c, SortWork& w, const uint32_t* keys_in, size_t n, int max_key_bits, const int* key_bits_dev) {
   return radix_sort_impl(c, w, keys_in, nullptr, n, max_key_bits, key_bits_dev, false, nullptr, nullptr);
 }

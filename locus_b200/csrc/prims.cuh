@@ -254,8 +254,9 @@ __device__ __forceinline__ void rs_reset_lookback(RsDev* rs, uint32_t* status, u
 int radix_sort_pairs(Ctx& c, SortWork& w, const uint32_t* keys_in, const uint32_t* vals_in, size_t n, int key_bits,
                      uint32_t** keys_out, uint32_t** vals_out);
 // The scatter passes only (val = element index), for a caller whose own key kernel filled the histogram
-// (rs_hist_warp_add / rs_hist_flush) and reset the look-back (rs_reset_lookback) after radix_sort_reserve.  The key
-// width is only known on the device: passes for max_key_bits are launched, those beyond *key_bits_dev return at once.
+// (rs_hist_warp_add / rs_hist_flush) and reset the look-back (rs_reset_lookback) after radix_sort_reserve.
+int radix_sort_scatter(Ctx& c, SortWork& w, const uint32_t* keys_in, size_t n, int key_bits, uint32_t** keys_out, uint32_t** vals_out);
+// The same when the key width is only known on the device: passes for max_key_bits are launched, those beyond *key_bits_dev return at once.
 // Result: buffers w.ka / w.va after an odd number of executed passes ((*key_bits_dev + 7) / 8), w.kb / w.vb after an
 // even number; consumers pick on the device.
 int radix_sort_pairs_devbits(Ctx& c, SortWork& w, const uint32_t* keys_in, size_t n, int max_key_bits, const int* key_bits_dev);
