@@ -478,6 +478,83 @@ int lb_submap_launch_count(lb_submap* m, uint64_t* n);
  * the k-NN covariance cache is used. */
 int lb_gicp_set_target_submap(lb_gicp* h, lb_submap* m);
 
+/* ------------------------------------------------------------------ NDT (SURVEY 8f row f4)
+ * LOCUS's alternative registration method (`registration_method: ndt`, registration_settings.h:3-12): the OpenMP NDT
+ * fork multithreaded_gicp/include/multithreaded_ndt/ndt_omp{.h,_impl.hpp} + voxel_grid_covariance_omp{.h,_impl.hpp},
+ * set up at PointCloudOdometry.cc:182-195 and PointCloudLocalization.cc:267-280 and then driven through the same
+ * icp_->setInputSource / setInputTarget / align / getFinalTransformation calls as GICP.
+ *
+ *   lb_ndt_create/destroy     make_shared<pclomp::NormalDistributionsTransform<PointF, PointF>>
+ *   lb_ndt_set_params         setTransformationEpsilon / setMaximumIterations / setResolution / setStepSize /
+ *                             setOulierRatio / setNeighborhoodSearchMethod (ndt_omp.h:124-196) and the voxel grid's
+ *                             setMinPointPerVoxel / setCovEigValueInflationRatio (voxel_grid_covariance_omp.h:203-236)
+ *   lb_ndt_set_source         icp_->setInputSource()
+ *   lb_ndt_set_target         icp_->setInputTarget() -> init() (ndt_omp.h:116-119,257-262): the target's voxel Gaussians
+ *   lb_ndt_align              icp_->align() + getFinalTransformation() + hasConverged() + getTransformationProbability()
+ *                             (computeTransformation, ndt_omp_impl.hpp:100-208)
+ *   lb_ndt_target_voxels      getTargetCells().getLeaves() restricted to the searchable voxels (voxel_centroids_ order)
+ *   lb_ndt_derivatives        computeDerivatives / computeHessian at a given pose (ndt_omp_impl.hpp:221-343,641-718)
+ *
+ * Semantics kept: non-finite target points are skipped; a source with a non-finite point is refused (previous source
+ * kept); a target whose int32 voxel index would overflow is refused (previous target kept); voxels with fewer than
+ * min_points_per_voxel points are not searchable; a voxel whose covariance fails the eigenvalue / inverse check stays in
+ * the radius search with nr_points = -1 exactly as in the reference (voxel_grid_covariance_omp_impl.hpp:326-355). */
+typedef struct lb_ndt lb_ndt;
+
+typedef struct lb_ndt_params {
+  float resolution;                 /* 1.0   voxel side and neighbour radius (ndt_omp_impl.hpp:50) */
+  double step_size;                 /* 0.1   More-Thuente maximum step (:51) */
+  double outlier_ratio;             /* 0.55  (:52) */
+  double transformation_epsilon;    /* 0.1   (:93); LOCUS passes icp_tf_epsilon / tf_epsilon */
+  int max_iterations;               /* 35    (:94); LOCUS passes icp_iterations / iterations */
+  int min_points_per_voxel;         /* 6     voxel_grid_covariance_omp.h:186 */
+  double min_covar_eigvalue_mult;   /* 0.01  voxel_grid_covariance_omp.h:187 */
+  int search_method;                /* 0 KDTREE (default, :96), 1 DIRECT26, 2 DIRECT7, 3 DIRECT1 (pclomp::NeighborSearchMethod values) */
+  /* accepted for interface compatibility (PointCloudOdometry.cc:189,191-193), no effect -- as in the reference's NDT */
+  double max_correspondence_distance;
+  int ransac_iterations;
+  int num_threads;
+  int enable_timing_output;
+} lb_ndt_params;
+
+typedef struct lb_ndt_result {
+  float final_transformation[16];   /* row-major 4x4 */
+  int converged;
+  int nr_iterations;
+  int n_evaluations;                /* computeDerivatives passes */
+  int n_target_voxels;              /* searchable voxels of the target */
+  double trans_probability;         /* score / source points (ndt_omp_impl.hpp:207) */
+  double pose[6];                   /* x y z roll pitch yaw of the last iterate */
+  double t_total_s;
+} lb_ndt_result;
+
+void lb_ndt_default_params(lb_ndt_params* p);
+int lb_ndt_create(int device, lb_ndt** h);
+int lb_ndt_create_on_stream(int device, void* cuda_stream, lb_ndt** h);
+int lb_ndt_destroy(lb_ndt* h);
+int lb_ndt_set_params(lb_ndt* h, const lb_ndt_params* p);
+int lb_ndt_set_source(lb_ndt* h, const void* pts, size_t n, size_t stride_bytes, size_t xyz_offset_bytes, int mem);
+int lb_ndt_set_target(lb_ndt* h, const void* pts, size_t n, size_t stride_bytes, size_t xyz_offset_bytes, int mem);
+/* The resident submap's current points as the target (the NDT counterpart of lb_gicp_set_target_submap; the map on the
+ * handle's device).  The points are gathered device to device into the handle's target, with no host copy; the voxel
+ * Gaussians are built lazily by the next align / derivatives / target_voxels, exactly as after lb_ndt_set_target of the
+ * same points (lb_submap_points order).  While the map's generation is unchanged a repeated call does no device work,
+ * so the Gaussians are rebuilt only after a keyframe insert or a crop.  After the map changed, align / derivatives /
+ * target_voxels refuse with LB_ERR_INVALID_ARG until the target is set again; the handle stays usable.  An empty map is
+ * LB_ERR_NO_TARGET, a map on another device LB_ERR_INVALID_ARG; the previous target is kept on any refusal. */
+int lb_ndt_set_target_submap(lb_ndt* h, lb_submap* m);
+/* guess16: row-major 4x4 float, NULL = identity (what LOCUS passes).  Blocking. */
+int lb_ndt_align(lb_ndt* h, const float* guess16, lb_ndt_result* result);
+/* host output buffers of `capacity` voxels each (any may be NULL); *n_voxels = searchable voxels, ascending voxel index */
+int lb_ndt_target_voxels(lb_ndt* h, size_t capacity, size_t* n_voxels, int32_t* leaf_idx, int32_t* nr_points, double* mean3,
+                         double* icov9, float* centroid3);
+/* sums over the source transformed by T16 (row-major 4x4), angle derivatives taken at pose6.  compute_hessian: 0 / 1 = the
+ * float path without / with the Hessian, 2 = the double-precision Hessian pass the line search ends with (score and
+ * gradient come back as 0). */
+int lb_ndt_derivatives(lb_ndt* h, const float* T16, const double* pose6, int compute_hessian, double* score, double* gradient6,
+                       double* hessian36);
+int lb_ndt_launch_count(lb_ndt* h, uint64_t* n);
+
 /* ------------------------------------------------- scan-to-scan odometry pipeline
  * One robot's lidar stream, scans submitted in order: VoxelGrid(scan k) -> GICP(source = filtered k, target =
  * filtered k-1), i.e. what Locus.cc:451-453 + PointCloudOdometry::UpdateEstimate do per scan.  Results are
@@ -498,9 +575,16 @@ typedef struct lb_odometry_result {
   int status;               /* lb_status of the stages of this scan */
   int has_pose;             /* 0 for the first scan (UpdateEstimate only stores it) or when a stage failed */
   size_t n_filtered;        /* points after VoxelGrid */
-  lb_gicp_result gicp;      /* as lb_gicp_align (valid when has_pose) */
+  lb_gicp_result gicp;      /* as lb_gicp_align (valid when has_pose).  Under LB_REG_NDT all zero except
+                               final_transformation, converged, iterations (= ndt.nr_iterations) and status, which carry
+                               the NDT align's values, so that a caller reading the pose needs no branch */
   char error[160];          /* message when status != LB_OK */
+  lb_ndt_result ndt;        /* as lb_ndt_align under LB_REG_NDT (valid when has_pose); zeros under LB_REG_GICP */
 } lb_odometry_result;
+
+/* the registration method of a pipeline (`registration_method: gicp | ndt`, PointCloudOdometry.cc:182-195,
+ * PointCloudLocalization.cc:267-280) */
+typedef enum lb_registration { LB_REG_GICP = 0, LB_REG_NDT = 1 } lb_registration;
 
 /* depth: registration workers (1..16).  max_points / max_point_step size the ring of filtered clouds. */
 int lb_odometry_create(int device, int depth, size_t max_points, uint32_t max_point_step, lb_odometry** out);
@@ -525,6 +609,14 @@ int lb_odometry_set_cloud_sharing(lb_odometry* h, int on);
  * gets its normals the same way.  Covariances come from them where the gicp params say recompute_*_covariance = 0.
  * Call while the pipeline is idle, before the first scan. */
 int lb_odometry_set_normals(lb_odometry* h, int k, const float* viewpoint);
+/* Registration method (LB_REG_GICP by default).  LB_REG_NDT: every worker owns an lb_ndt handle (own stream) and
+ * registration k is lb_ndt_set_source(filtered k) + lb_ndt_set_target(filtered k-1) + lb_ndt_align(prior), i.e. what the
+ * blocking lb_ndt_* calls give; `ndt` (validated as lb_ndt_set_params does) is applied to every worker.  Cloud sharing is
+ * a GICP concept and is ignored under NDT; the normals stage has no consumer there, so NDT together with normals k > 0 is
+ * refused (LB_ERR_UNSUPPORTED) whichever of the two calls comes second.  Call while the pipeline is idle; a method
+ * change after the first scan is refused (LB_ERR_UNSUPPORTED).  ndt may be NULL with LB_REG_GICP.  Any refusal leaves
+ * the previous setting in place. */
+int lb_odometry_set_registration(lb_odometry* h, int method, const lb_ndt_params* ndt);
 /* scan: n_pts points of point_step bytes described by fields (as lb_voxel_filter); xyz must be FLOAT32 fields.
  * guess: row-major 4x4 prior handed to align() (NULL = identity).  filtered_out (nullable): host (LB_MEM_HOST) or
  * device buffer of at least n_pts * point_step bytes that receives the filtered cloud.  Blocks while 2*depth+2 scans
@@ -623,6 +715,15 @@ typedef struct lb_locus_params {
   double initial_pose[16];               /* row-major; L and the last keyframe before the first scan */
   lb_locus_front_end front_end;          /* normals and adaptive input voxelization (off by default) */
   lb_locus_icp_covariance icp_covariance;   /* the localization's ICP covariance (off by default) */
+  /* registration_method of each package (LB_REG_GICP by default; fixed after the first scan).  Odometry NDT registers
+   * filtered k against filtered k-1 with odometry_ndt; the scan's GICP cloud is still prepared and shared for the
+   * localization stage (keyframe transform, ICP covariance, GICP localization), with the `odometry` GICP params.
+   * Localization NDT aligns the scan's filtered points against the submap's points (lb_ndt_set_target_submap) with
+   * localization_ndt; the ICP covariance, when enabled, is computed on the NDT pose against the submap.  An NDT params
+   * block is validated (as lb_ndt_set_params) only when its method is NDT.  Defaults: lb_ndt_default_params with
+   * transformation_epsilon / max_iterations of the packages' parameters.yaml: odometry 1e-3 / 20, localization 1e-5 / 20. */
+  int odometry_method, localization_method;
+  lb_ndt_params odometry_ndt, localization_ndt;
 } lb_locus_params;
 
 typedef struct lb_locus_result {
@@ -654,6 +755,9 @@ typedef struct lb_locus_result {
                                       fallbacks from the start: the reference publishes an uninitialised value there);
                                       0 when icp_covariance is off */
   int icp_covariance_flags;        /* LB_ICPCOV_* */
+  /* the NDT aligns' results under LB_REG_NDT (zeros under GICP); `odometry` / `localization` then carry their
+   * final_transformation, converged, iterations and status as in lb_odometry_result */
+  lb_ndt_result odometry_ndt, localization_ndt;
 } lb_locus_result;
 
 /* the reference's shipped values: locus/config/lo_settings.yaml, point_cloud_odometry/config/parameters.yaml,
@@ -665,7 +769,8 @@ int lb_locus_create(int device, int depth, size_t max_points, uint32_t max_point
 int lb_locus_destroy(lb_locus* h);
 lb_voxel* lb_locus_voxel(lb_locus* h);
 /* refused while scans are in flight, when the two gicp params disagree on the shared clouds, when front_end is out of
- * range, and when normals_k changes after the first scan; the previous parameters stay in place */
+ * range, when normals_k or a registration method changes after the first scan, and when the NDT params of a method set
+ * to NDT are invalid; the previous parameters stay in place */
 int lb_locus_set_params(lb_locus* h, const lb_locus_params* p);
 /* same arguments and blocking rule as lb_odometry_submit; guess = the odometry prior */
 int lb_locus_submit(lb_locus* h, const uint8_t* scan, size_t n_pts, uint32_t point_step, const lb_field* fields,
@@ -679,75 +784,6 @@ int lb_locus_next(lb_locus* h, lb_locus_result* r, int block);
 int lb_locus_pending(lb_locus* h, size_t* n);
 /* out9 = the six values of lb_odometry_stage_times, then { scans localized, localization stage busy s, its wait s } */
 int lb_locus_stage_times(lb_locus* h, double* out9);
-
-/* ------------------------------------------------------------------ NDT (SURVEY 8f row f4)
- * LOCUS's alternative registration method (`registration_method: ndt`, registration_settings.h:3-12): the OpenMP NDT
- * fork multithreaded_gicp/include/multithreaded_ndt/ndt_omp{.h,_impl.hpp} + voxel_grid_covariance_omp{.h,_impl.hpp},
- * set up at PointCloudOdometry.cc:182-195 and PointCloudLocalization.cc:267-280 and then driven through the same
- * icp_->setInputSource / setInputTarget / align / getFinalTransformation calls as GICP.
- *
- *   lb_ndt_create/destroy     make_shared<pclomp::NormalDistributionsTransform<PointF, PointF>>
- *   lb_ndt_set_params         setTransformationEpsilon / setMaximumIterations / setResolution / setStepSize /
- *                             setOulierRatio / setNeighborhoodSearchMethod (ndt_omp.h:124-196) and the voxel grid's
- *                             setMinPointPerVoxel / setCovEigValueInflationRatio (voxel_grid_covariance_omp.h:203-236)
- *   lb_ndt_set_source         icp_->setInputSource()
- *   lb_ndt_set_target         icp_->setInputTarget() -> init() (ndt_omp.h:116-119,257-262): the target's voxel Gaussians
- *   lb_ndt_align              icp_->align() + getFinalTransformation() + hasConverged() + getTransformationProbability()
- *                             (computeTransformation, ndt_omp_impl.hpp:100-208)
- *   lb_ndt_target_voxels      getTargetCells().getLeaves() restricted to the searchable voxels (voxel_centroids_ order)
- *   lb_ndt_derivatives        computeDerivatives / computeHessian at a given pose (ndt_omp_impl.hpp:221-343,641-718)
- *
- * Semantics kept: non-finite target points are skipped; a source with a non-finite point is refused (previous source
- * kept); a target whose int32 voxel index would overflow is refused (previous target kept); voxels with fewer than
- * min_points_per_voxel points are not searchable; a voxel whose covariance fails the eigenvalue / inverse check stays in
- * the radius search with nr_points = -1 exactly as in the reference (voxel_grid_covariance_omp_impl.hpp:326-355). */
-typedef struct lb_ndt lb_ndt;
-
-typedef struct lb_ndt_params {
-  float resolution;                 /* 1.0   voxel side and neighbour radius (ndt_omp_impl.hpp:50) */
-  double step_size;                 /* 0.1   More-Thuente maximum step (:51) */
-  double outlier_ratio;             /* 0.55  (:52) */
-  double transformation_epsilon;    /* 0.1   (:93); LOCUS passes icp_tf_epsilon / tf_epsilon */
-  int max_iterations;               /* 35    (:94); LOCUS passes icp_iterations / iterations */
-  int min_points_per_voxel;         /* 6     voxel_grid_covariance_omp.h:186 */
-  double min_covar_eigvalue_mult;   /* 0.01  voxel_grid_covariance_omp.h:187 */
-  int search_method;                /* 0 KDTREE (default, :96), 1 DIRECT26, 2 DIRECT7, 3 DIRECT1 (pclomp::NeighborSearchMethod values) */
-  /* accepted for interface compatibility (PointCloudOdometry.cc:189,191-193), no effect -- as in the reference's NDT */
-  double max_correspondence_distance;
-  int ransac_iterations;
-  int num_threads;
-  int enable_timing_output;
-} lb_ndt_params;
-
-typedef struct lb_ndt_result {
-  float final_transformation[16];   /* row-major 4x4 */
-  int converged;
-  int nr_iterations;
-  int n_evaluations;                /* computeDerivatives passes */
-  int n_target_voxels;              /* searchable voxels of the target */
-  double trans_probability;         /* score / source points (ndt_omp_impl.hpp:207) */
-  double pose[6];                   /* x y z roll pitch yaw of the last iterate */
-  double t_total_s;
-} lb_ndt_result;
-
-void lb_ndt_default_params(lb_ndt_params* p);
-int lb_ndt_create(int device, lb_ndt** h);
-int lb_ndt_create_on_stream(int device, void* cuda_stream, lb_ndt** h);
-int lb_ndt_destroy(lb_ndt* h);
-int lb_ndt_set_params(lb_ndt* h, const lb_ndt_params* p);
-int lb_ndt_set_source(lb_ndt* h, const void* pts, size_t n, size_t stride_bytes, size_t xyz_offset_bytes, int mem);
-int lb_ndt_set_target(lb_ndt* h, const void* pts, size_t n, size_t stride_bytes, size_t xyz_offset_bytes, int mem);
-/* guess16: row-major 4x4 float, NULL = identity (what LOCUS passes).  Blocking. */
-int lb_ndt_align(lb_ndt* h, const float* guess16, lb_ndt_result* result);
-/* host output buffers of `capacity` voxels each (any may be NULL); *n_voxels = searchable voxels, ascending voxel index */
-int lb_ndt_target_voxels(lb_ndt* h, size_t capacity, size_t* n_voxels, int32_t* leaf_idx, int32_t* nr_points, double* mean3,
-                         double* icov9, float* centroid3);
-/* sums over the source transformed by T16 (row-major 4x4), angle derivatives taken at pose6.  compute_hessian: 0 / 1 = the
- * float path without / with the Hessian, 2 = the double-precision Hessian pass the line search ends with (score and
- * gradient come back as 0). */
-int lb_ndt_derivatives(lb_ndt* h, const float* T16, const double* pose6, int compute_hessian, double* score, double* gradient6,
-                       double* hessian36);
-int lb_ndt_launch_count(lb_ndt* h, uint64_t* n);
 
 #ifdef __cplusplus
 }

@@ -71,7 +71,16 @@ class NdtResult(C.Structure):
 
 class OdometryResult(C.Structure):
     _fields_ = [("ticket", C.c_uint64), ("status", C.c_int), ("has_pose", C.c_int), ("n_filtered", C.c_size_t),
-                ("gicp", GicpResult), ("error", C.c_char * 160)]
+                ("gicp", GicpResult), ("error", C.c_char * 160), ("ndt", NdtResult)]
+
+
+# lb_registration: a pipeline's registration method (registration_method: gicp | ndt)
+LB_REG_GICP, LB_REG_NDT = 0, 1
+_REG = {"gicp": LB_REG_GICP, "ndt": LB_REG_NDT}
+
+
+def _reg_method(m):
+    return _REG[m] if isinstance(m, str) else int(m)
 
 
 class LocusThresholds(C.Structure):
@@ -92,7 +101,8 @@ class LocusParams(C.Structure):
                 ("localization_thresholds", LocusThresholds), ("translation_threshold_kf", C.c_double),
                 ("rotation_threshold_kf", C.c_double), ("add_keyframes", C.c_int), ("refresh_every", C.c_int),
                 ("msw", C.c_int), ("window_half_size", C.c_float), ("prior_map", C.c_int), ("initial_pose", C.c_double * 16),
-                ("front_end", LocusFrontEnd), ("icp_covariance", LocusIcpCovariance)]
+                ("front_end", LocusFrontEnd), ("icp_covariance", LocusIcpCovariance), ("odometry_method", C.c_int),
+                ("localization_method", C.c_int), ("odometry_ndt", NdtParams), ("localization_ndt", NdtParams)]
 
 
 class LocusResult(C.Structure):
@@ -102,7 +112,8 @@ class LocusResult(C.Structure):
                 ("odometry_pose", C.c_double * 16), ("incremental", C.c_double * 16), ("pose", C.c_double * 16),
                 ("keyframe", C.c_int), ("n_inserted", C.c_size_t), ("n_removed", C.c_size_t), ("map_size", C.c_size_t),
                 ("leaf_size", C.c_float), ("has_icp_covariance", C.c_int), ("icp_covariance", C.c_double * 36),
-                ("condition_number", C.c_double), ("icp_covariance_flags", C.c_int)]
+                ("condition_number", C.c_double), ("icp_covariance_flags", C.c_int), ("odometry_ndt", NdtResult),
+                ("localization_ndt", NdtResult)]
 
 
 # lb_icp_covariance.flags
@@ -154,12 +165,13 @@ SYMBOLS = [
     "lb_submap_create", "lb_submap_destroy", "lb_submap_clear", "lb_submap_insert", "lb_submap_crop_box", "lb_submap_size",
     "lb_submap_generation", "lb_submap_points", "lb_submap_insert_with_normals", "lb_submap_normals", "lb_submap_neighbors", "lb_submap_launch_count", "lb_gicp_set_target_submap",
     "lb_odometry_create", "lb_odometry_destroy", "lb_odometry_voxel", "lb_odometry_gicp", "lb_odometry_depth",
-    "lb_odometry_set_gicp_params", "lb_odometry_set_cloud_sharing", "lb_odometry_set_normals", "lb_odometry_submit", "lb_odometry_next", "lb_odometry_pending",
+    "lb_odometry_set_gicp_params", "lb_odometry_set_cloud_sharing", "lb_odometry_set_normals", "lb_odometry_set_registration", "lb_odometry_submit", "lb_odometry_next", "lb_odometry_pending",
     "lb_odometry_launch_count", "lb_odometry_stage_times", "lb_odometry_submit_merged",
     "lb_locus_default_params", "lb_locus_create", "lb_locus_destroy", "lb_locus_voxel", "lb_locus_set_params", "lb_locus_submit",
     "lb_locus_next", "lb_locus_pending", "lb_locus_stage_times", "lb_locus_submit_merged",
     "lb_ndt_default_params", "lb_ndt_create", "lb_ndt_create_on_stream", "lb_ndt_destroy", "lb_ndt_set_params", "lb_ndt_set_source",
     "lb_ndt_set_target", "lb_ndt_align", "lb_ndt_target_voxels", "lb_ndt_derivatives", "lb_ndt_launch_count",
+    "lb_ndt_set_target_submap",
 ]
 
 
@@ -283,6 +295,8 @@ def lib():
             L.lb_odometry_set_cloud_sharing.argtypes = [vp, i32]
         if hasattr(L, "lb_odometry_set_normals"):
             L.lb_odometry_set_normals.argtypes = [vp, i32, vp]
+        if hasattr(L, "lb_odometry_set_registration"):
+            L.lb_odometry_set_registration.argtypes = [vp, i32, C.POINTER(NdtParams)]
         L.lb_odometry_submit.argtypes = [vp, vp, sz, C.c_uint32, C.POINTER(Field), i32, i32, vp, vp, i32, u64p]
         L.lb_odometry_next.argtypes = [vp, C.POINTER(OdometryResult), i32]
         L.lb_odometry_pending.argtypes = [vp, C.POINTER(sz)]
@@ -317,6 +331,8 @@ def lib():
         L.lb_ndt_target_voxels.argtypes = [vp, sz, C.POINTER(sz), vp, vp, vp, vp, vp]
         L.lb_ndt_derivatives.argtypes = [vp, vp, vp, i32, C.POINTER(C.c_double), vp, vp]
         L.lb_ndt_launch_count.argtypes = [vp, u64p]
+        if hasattr(L, "lb_ndt_set_target_submap"):
+            L.lb_ndt_set_target_submap.argtypes = [vp, vp]
     _lib = L
     return L
 
@@ -940,6 +956,17 @@ class OdometryB200:
         vp_ = None if viewpoint is None else np.ascontiguousarray(viewpoint, dtype=np.float32)
         _check(lib().lb_odometry_set_normals(self._h, int(k), _ptr(vp_)))
 
+    def setRegistration(self, method="ndt", **ndt):
+        """registration method of every worker: "gicp" (default) or "ndt"; keywords = lb_ndt_params fields over
+        lb_ndt_default_params (idle pipeline; the method is fixed once the first scan is submitted)"""
+        p = NdtParams()
+        lib().lb_ndt_default_params(C.byref(p))
+        for k, v in ndt.items():
+            if not hasattr(p, k):
+                raise AttributeError(k)
+            setattr(p, k, v)
+        _check(lib().lb_odometry_set_registration(self._h, _reg_method(method), C.byref(p)))
+
     def submit(self, scan, n_pts, point_step, fields, mem=LB_MEM_HOST, guess=None, filtered_out=None,
                mem_filtered=LB_MEM_HOST):
         """scan / filtered_out: host uint8 numpy arrays or raw pointers (int).  Returns the ticket."""
@@ -995,7 +1022,8 @@ class OdometryB200:
 
 def locus_params(**kw):
     """lb_locus_params with the reference's shipped values; keywords override top-level fields, and `odometry` /
-    `localization` / `*_thresholds` / `front_end` / `icp_covariance` take dicts of their fields"""
+    `localization` / `*_thresholds` / `front_end` / `icp_covariance` / `*_ndt` take dicts of their fields;
+    `odometry_method` / `localization_method` take "gicp" or "ndt" (or LB_REG_*)"""
     p = LocusParams()
     _check(lib().lb_locus_default_params(C.byref(p)))
     for k, v in kw.items():
@@ -1012,6 +1040,8 @@ def locus_params(**kw):
                     setattr(sub, kk, vv)
         elif k == "initial_pose":
             p.initial_pose[:] = [float(x) for x in np.asarray(v, dtype=np.float64).reshape(16)]
+        elif k in ("odometry_method", "localization_method"):
+            setattr(p, k, _reg_method(v))
         else:
             setattr(p, k, v)
     return p
@@ -1162,6 +1192,11 @@ class NdtB200:
     def setInputTarget(self, cloud):
         a = self._cloud(cloud)
         _check(lib().lb_ndt_set_target(self._h, _ptr(a), a.shape[0], a.shape[1] * 4, 0, LB_MEM_HOST))
+
+    def setTargetSubmap(self, submap):
+        """the SubmapB200's current points as the target, gathered on the device (lb_ndt_set_target_submap); call again
+        after the map changed -- while it is unchanged the call does nothing"""
+        _check(lib().lb_ndt_set_target_submap(self._h, submap._h))
 
     def align(self, guess=None):
         g = None if guess is None else np.ascontiguousarray(guess, dtype=np.float32).reshape(16)

@@ -30,6 +30,10 @@
 
 namespace lb {
 
+// the resident submap (submap.cuh, compiled into gicp.cu): its current points, count, generation and stream
+int submap_device(const lb_submap* m);
+void submap_points_view(const lb_submap* m, const f4** pts, size_t* n, uint64_t* generation, cudaStream_t* stream);
+
 constexpr int NDT_EVAL_THREADS = 128;
 constexpr int NDT_BATCH = 8;            // [evaluation, controller] steps enqueued between two looks at the controller
 
@@ -481,6 +485,9 @@ struct lb_ndt {
   float tgt_mn[3] = {0, 0, 0}, tgt_mx[3] = {0, 0, 0};
   bool tgt_dirty = false;               // the voxel structure has to be (re)built from tgt
   bool have_tgt = false;
+  const lb_submap* tgt_map = nullptr;   // lb_ndt_set_target_submap: the map tgt was gathered from, at this generation
+  uint64_t tgt_map_gen = 0;
+  cudaEvent_t map_ready = nullptr;      // the map's stream -> this handle's stream
   DBuf<uint32_t> keys, flag, slot_of, head_pos;
   SortWork sort;
   ScanWork scan;
@@ -569,23 +576,36 @@ int lb_ndt_destroy(lb_ndt* h) {
   if (h->h_acc) cudaFreeHost(h->h_acc);
   if (h->d_u32) cudaFree(h->d_u32);
   if (h->h_u32) cudaFreeHost(h->h_u32);
+  if (h->map_ready) cudaEventDestroy(h->map_ready);
   ctx_destroy(h->c);
   delete h;
   return LB_OK;
 }
 
-int lb_ndt_set_params(lb_ndt* h, const lb_ndt_params* p) {
-  if (!h || !p) { set_error("lb_ndt_set_params: null argument"); return LB_ERR_INVALID_ARG; }
+}  // extern "C"
+
+namespace lb {
+// lb_ndt_set_params' refusals, shared with the pipelines that take NDT params (odometry.cu)
+int ndt_check_params(const lb_ndt_params* p, const char* who) {
   if (!(p->resolution > 0) || !(p->step_size > 0) || !(p->outlier_ratio > 0) || !(p->outlier_ratio < 1) ||
       !(p->transformation_epsilon > 0) || p->max_iterations < 0 || p->min_points_per_voxel < 3 || !(p->min_covar_eigvalue_mult > 0)) {
     // setMinPointVoxel refuses fewer than 3 points (voxel_grid_covariance_omp.h:203-214)
-    set_error("lb_ndt_set_params: resolution / step / outlier ratio / epsilon must be positive, min_points_per_voxel >= 3");
+    set_error("%s: resolution / step / outlier ratio / epsilon must be positive, min_points_per_voxel >= 3", who);
     return LB_ERR_INVALID_ARG;
   }
   if (p->search_method < NDT_KDTREE || p->search_method > NDT_DIRECT1) {
-    set_error("lb_ndt_set_params: search_method must be 0 (KDTREE), 1 (DIRECT26), 2 (DIRECT7) or 3 (DIRECT1)");
+    set_error("%s: search_method must be 0 (KDTREE), 1 (DIRECT26), 2 (DIRECT7) or 3 (DIRECT1)", who);
     return LB_ERR_UNSUPPORTED;
   }
+  return LB_OK;
+}
+}  // namespace lb
+
+extern "C" {
+
+int lb_ndt_set_params(lb_ndt* h, const lb_ndt_params* p) {
+  if (!h || !p) { set_error("lb_ndt_set_params: null argument"); return LB_ERR_INVALID_ARG; }
+  LB_TRY(ndt_check_params(p, "lb_ndt_set_params"));
   // setResolution re-initialises the voxel structure of the current target (ndt_omp.h:124-131); the same holds for the
   // two voxel parameters
   if (p->resolution != h->P.resolution || p->min_points_per_voxel != h->P.min_points_per_voxel ||
@@ -634,17 +654,16 @@ int lb_ndt_set_source(lb_ndt* h, const void* pts, size_t n, size_t stride, size_
   return LB_OK;
 }
 
-int lb_ndt_set_target(lb_ndt* h, const void* pts, size_t n, size_t stride, size_t xyz_off, int mem) {
-  if (!h) { set_error("lb_ndt_set_target: null handle"); return LB_ERR_INVALID_ARG; }
-  if (n == 0) { set_error("lb_ndt_set_target: empty target cloud"); return LB_ERR_NO_TARGET; }
-  LB_TRY(ndt_upload(h, h->tgt_spare, pts, n, stride, xyz_off, mem, "lb_ndt_set_target"));
-  if (h->h_acc->count == 0) { set_error("lb_ndt_set_target: no finite point; the previous target is kept"); return LB_ERR_NO_TARGET; }
+// lb_ndt_set_target and lb_ndt_set_target_submap: upload into the spare buffer, then swap (any refusal keeps the target)
+static int ndt_take_target(lb_ndt* h, const void* pts, size_t n, size_t stride, size_t xyz_off, int mem, const char* who) {
+  LB_TRY(ndt_upload(h, h->tgt_spare, pts, n, stride, xyz_off, mem, who));
+  if (h->h_acc->count == 0) { set_error("%s: no finite point; the previous target is kept", who); return LB_ERR_NO_TARGET; }
   // lattice check before the swap: a grid the reference would refuse leaves the previous target in place
   float mn[3], mx[3];
   for (int a = 0; a < 3; a++) { mn[a] = ord2f(h->h_acc->mn[a]); mx[a] = ord2f(h->h_acc->mx[a]); }
   NdtLattice L;
   if (!ndt_lattice(mn, mx, h->P.resolution, L)) {
-    set_error("lb_ndt_set_target: leaf size is too small for the input dataset, integer indices would overflow");
+    set_error("%s: leaf size is too small for the input dataset, integer indices would overflow", who);
     return LB_ERR_VOXEL_OVERFLOW;
   }
   std::swap(h->tgt, h->tgt_spare);
@@ -652,6 +671,39 @@ int lb_ndt_set_target(lb_ndt* h, const void* pts, size_t n, size_t stride, size_
   h->n_tgt = (uint32_t)n;
   h->tgt_dirty = true;
   h->have_tgt = false;
+  h->tgt_map = nullptr;
+  return LB_OK;
+}
+
+int lb_ndt_set_target(lb_ndt* h, const void* pts, size_t n, size_t stride, size_t xyz_off, int mem) {
+  if (!h) { set_error("lb_ndt_set_target: null handle"); return LB_ERR_INVALID_ARG; }
+  if (n == 0) { set_error("lb_ndt_set_target: empty target cloud"); return LB_ERR_NO_TARGET; }
+  return ndt_take_target(h, pts, n, stride, xyz_off, mem, "lb_ndt_set_target");
+}
+
+int lb_ndt_set_target_submap(lb_ndt* h, lb_submap* m) {
+  if (!h || !m) { set_error("lb_ndt_set_target_submap: null argument"); return LB_ERR_INVALID_ARG; }
+  if (submap_device(m) != h->c.device) {
+    set_error("lb_ndt_set_target_submap: submap on device %d, handle on %d", submap_device(m), h->c.device);
+    return LB_ERR_INVALID_ARG;
+  }
+  const f4* pts = nullptr;
+  size_t n = 0;
+  uint64_t gen = 0;
+  cudaStream_t map_stream = nullptr;
+  submap_points_view(m, &pts, &n, &gen, &map_stream);
+  if (h->tgt_map == m && h->tgt_map_gen == gen) return LB_OK;      // unchanged map: the target (and its Gaussians) stand
+  if (n == 0) { set_error("lb_ndt_set_target_submap: the map is empty"); return LB_ERR_NO_TARGET; }
+  LB_CUDA(cudaSetDevice(h->c.device));
+  // The gather reads the map's buffer on this handle's stream: an event recorded on the map's stream orders it after
+  // whatever map work is still pending there (the map calls synchronise before they return today; the event keeps
+  // that an implementation detail of the map).
+  if (!h->map_ready) LB_CUDA(cudaEventCreateWithFlags(&h->map_ready, cudaEventDisableTiming));
+  LB_CUDA(cudaEventRecord(h->map_ready, map_stream));
+  LB_CUDA(cudaStreamWaitEvent(h->c.stream, h->map_ready, 0));
+  LB_TRY(ndt_take_target(h, pts, n, sizeof(f4), 0, LB_MEM_DEVICE, "lb_ndt_set_target_submap"));
+  h->tgt_map = m;
+  h->tgt_map_gen = gen;
   return LB_OK;
 }
 
@@ -710,6 +762,17 @@ static int ndt_ready(lb_ndt* h, const char* who) {
   if (!h) { set_error("%s: null handle", who); return LB_ERR_INVALID_ARG; }
   LB_CUDA(cudaSetDevice(h->c.device));
   if (h->n_tgt == 0) { set_error("%s: no target set", who); return LB_ERR_NO_TARGET; }
+  if (h->tgt_map) {
+    const f4* pts = nullptr;
+    size_t n = 0;
+    uint64_t gen = 0;
+    cudaStream_t st = nullptr;
+    submap_points_view(h->tgt_map, &pts, &n, &gen, &st);
+    if (gen != h->tgt_map_gen) {
+      set_error("%s: the map changed since lb_ndt_set_target_submap; call it again", who);
+      return LB_ERR_INVALID_ARG;
+    }
+  }
   if (h->tgt_dirty || !h->have_tgt) LB_TRY(ndt_build_target(h));
   h->tv.method = h->P.search_method;
   h->tv.min_pts = h->P.min_points_per_voxel;
@@ -820,3 +883,28 @@ int lb_ndt_launch_count(lb_ndt* h, uint64_t* n) {
 }
 
 }  // extern "C"
+
+namespace lb {
+
+// Pre-sizes every buffer an NDT registration of clouds of up to max_points device-resident points touches (source,
+// target, voxel build, sort, scan, evaluation partials), so that lb_odometry's workers make no device allocation in
+// steady state.  The host upload staging is not reserved: the pipelines hand device clouds only.
+int ndt_reserve(lb_ndt* h, size_t max_points) {
+  if (!h || max_points == 0 || max_points > 0x7fffffffull) { set_error("ndt_reserve: bad argument"); return LB_ERR_INVALID_ARG; }
+  LB_CUDA(cudaSetDevice(h->c.device));
+  const size_t n = max_points;
+  LB_TRY(h->src.ensure(n)); LB_TRY(h->src_spare.ensure(n)); LB_TRY(h->tgt.ensure(n)); LB_TRY(h->tgt_spare.ensure(n));
+  LB_TRY(h->keys.ensure(n)); LB_TRY(h->flag.ensure(n)); LB_TRY(h->slot_of.ensure(n));
+  LB_TRY(radix_sort_reserve(h->c, h->sort, n));
+  LB_TRY(h->scan.sums.ensure(std::max<size_t>((n + 2047) / 2048, 16384)));    // exclusive_scan_u32's spine
+  LB_TRY(h->vox.ensure(n + 1)); LB_TRY(h->cen.ensure(n + 1)); LB_TRY(h->leaf_idx.ensure(n + 1)); LB_TRY(h->head_pos.ensure(n + 1));
+  uint32_t cap = 16;
+  while (cap < 2u * (uint32_t)n) cap <<= 1;                           // ndt_build_target's table for n searchable voxels
+  LB_TRY(h->hkey.ensure(cap)); LB_TRY(h->hval.ensure(cap));
+  const size_t rows = std::max(cdiv((long long)n, NDT_EVAL_THREADS), cdiv((long long)n, NDT_GPTS * NDT_GBATCH));
+  LB_TRY(h->partials.ensure(rows * NDT_NSUM));
+  LB_CUDA(cudaStreamSynchronize(h->c.stream));
+  return LB_OK;
+}
+
+}  // namespace lb

@@ -6,7 +6,8 @@
 //   stage V  one thread, one lb_voxel handle (own stream): VoxelGrid of scan k into slot k % R of a ring of
 //            device-resident filtered clouds
 //   stage G  `depth` threads, one lb_gicp handle each (own streams): set_source(ring[k]), set_target(ring[k-1]),
-//            align -> result k
+//            align -> result k; under LB_REG_NDT (lb_odometry_set_registration) the same three calls on the worker's
+//            lb_ndt handle instead
 //
 // Nothing here touches a point: every byte of device work is done by voxel.cu / gicp.cu kernels.  The pipeline
 // exists because one align() is a chain of latency-bound kernels on a fraction of the SMs: the rest of the GPU filters
@@ -32,14 +33,18 @@
 #include "front_end_stub.h"
 #include "icp_covariance_stub.h"
 #include "merged_stub.h"
+#include "ndt_stub.h"
 #elif defined(LB_ODOMETRY_STUB)  // TEST-ONLY build without CUDA: tests/odometry_harness.cpp supplies fake stages
 #include "odometry_stub.h"
 #include "front_end_stub.h"
 #include "merged_stub.h"
+#include "ndt_stub.h"
 #else
 #include "prims.cuh"
 namespace lb {
 int voxel_reserve(lb_voxel* h, size_t n_pts, uint32_t max_step);   // voxel.cu
+int ndt_reserve(lb_ndt* h, size_t max_points);                       // ndt.cu
+int ndt_check_params(const lb_ndt_params* p, const char* who);      // ndt.cu
 }
 #endif
 #include "lo_pose.h"
@@ -112,6 +117,8 @@ struct lb_odometry {
   bool chain = false;                  // run by lb_locus: stage L completes the tickets
   int normals_k = 0;                   // lb_odometry_set_normals (0 = off)
   float normals_vp[3] = {0.f, 0.f, 0.f};
+  int method = LB_REG_GICP;            // lb_odometry_set_registration
+  std::vector<lb_ndt*> ndt;            // one per worker (own streams), created when NDT is first selected
   // lb_locus's adaptive input voxelization (Locus.cc:780-810), touched by stage V only (and by lb_locus_set_params
   // while nothing is in flight)
   bool adaptive = false;
@@ -146,6 +153,16 @@ void copy_err(char* dst, size_t cap) {
   const char* e = lb_last_error_string();
   strncpy(dst, e ? e : "", cap - 1);
   dst[cap - 1] = 0;
+}
+
+// what lb_odometry_result.gicp (and lb_locus_result.odometry / .localization) carry under NDT: the pose, converged,
+// iterations and status; every other field 0
+void ndt_as_gicp(const lb_ndt_result& n, lb_gicp_result& g) {
+  memset(&g, 0, sizeof(g));
+  memcpy(g.final_transformation, n.final_transformation, sizeof(g.final_transformation));
+  g.converged = n.converged;
+  g.iterations = n.nr_iterations;
+  g.status = LB_OK;
 }
 
 void advance_done_floor(lb_odometry* h) {   // mu held
@@ -257,7 +274,26 @@ void align_stage(lb_odometry* h, int w) {
     const Slot& cur = h->ring[t % R];
     r.status = cur.status;
     if (cur.status != LB_OK) memcpy(r.error, cur.error, sizeof(r.error));
-    if (h->share) {
+    if (h->method == LB_REG_NDT) {
+      if (h->chain && cur.status == LB_OK && cur.n > 0) {
+        // stage L still takes this scan's GICP cloud (keyframe transform, ICP covariance, a GICP localization): prepared
+        // here, off stage L's critical path, with the odometry GICP params
+        int st = lb_gicp_set_source(g, cur.d, cur.n, cur.point_step, (size_t)cur.xyz_off, LB_NO_NORMALS, LB_MEM_DEVICE);
+        if (st == LB_OK && h->normals_k) st = lb_gicp_estimate_normals(g, 0, h->normals_k, h->normals_vp);
+        if (st == LB_OK) st = lb_gicp_prepare_source(g);
+        if (st == LB_OK) st = lb_gicp_share_source(g, &e->loc_cloud);
+        if (st != LB_OK) { r.status = st; copy_err(r.error, sizeof(r.error)); }
+      }
+      const Slot& prv = h->ring[(t + R - 1) % R];
+      if (t > 0 && r.status == LB_OK && prv.status == LB_OK && prv.n > 0 && cur.n > 0) {
+        lb_ndt* nd = h->ndt[(size_t)w];
+        int st = lb_ndt_set_source(nd, cur.d, cur.n, cur.point_step, (size_t)cur.xyz_off, LB_MEM_DEVICE);
+        if (st == LB_OK) st = lb_ndt_set_target(nd, prv.d, prv.n, prv.point_step, (size_t)prv.xyz_off, LB_MEM_DEVICE);
+        if (st == LB_OK) st = lb_ndt_align(nd, e->job.has_guess ? e->job.guess : nullptr, &r.ndt);
+        r.status = st;
+        if (st == LB_OK) { r.has_pose = 1; ndt_as_gicp(r.ndt, r.gicp); } else copy_err(r.error, sizeof(r.error));
+      }
+    } else if (h->share) {
       // this scan's cloud is prepared here, once, and published for the worker of the next registration
       lb_cloud* mine = nullptr;
       int st = cur.status;
@@ -387,6 +423,59 @@ int odometry_create(int device, int depth, size_t max_points, uint32_t max_point
   return LB_OK;
 }
 
+// The refusals of a registration setting, before anything changes (mu not held): method, NDT params, an idle pipeline,
+// a method change after the first scan, and NDT with the normals stage outside lb_locus.
+int registration_check(lb_odometry* h, int method, const lb_ndt_params* ndt, const char* who) {
+  if (method != LB_REG_GICP && method != LB_REG_NDT) {
+    set_error("%s: method must be LB_REG_GICP (0) or LB_REG_NDT (1), got %d", who, method);
+    return LB_ERR_INVALID_ARG;
+  }
+  if (method == LB_REG_NDT) {
+    if (!ndt) { set_error("%s: NDT needs its params", who); return LB_ERR_INVALID_ARG; }
+    LB_TRY(ndt_check_params(ndt, who));
+  }
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (h->next_return != h->next_ticket) { set_error("%s: pipeline not idle", who); return LB_ERR_INVALID_ARG; }
+  if (h->next_ticket != 0 && method != h->method) {
+    // the previous scan exists only in the form its method prepared (a GICP worker adopts its shared cloud)
+    set_error("%s: change the registration method before the first scan is submitted", who);
+    return LB_ERR_UNSUPPORTED;
+  }
+  if (method == LB_REG_NDT && h->normals_k && !h->chain) {
+    set_error("%s: the normals stage has no consumer under NDT registration", who);
+    return LB_ERR_UNSUPPORTED;
+  }
+  return LB_OK;
+}
+
+// one lb_ndt per worker, sized like the ring, created the first time NDT is selected
+int odometry_ndt_handles(lb_odometry* h) {
+  if (!h->ndt.empty()) return LB_OK;
+  std::vector<lb_ndt*> v;
+  int st = LB_OK;
+  for (int i = 0; st == LB_OK && i < h->depth; i++) {
+    lb_ndt* n = nullptr;
+    st = lb_ndt_create(h->device, &n);
+    if (st == LB_OK) v.push_back(n);
+    if (st == LB_OK) st = ndt_reserve(n, h->max_points);
+  }
+  if (st != LB_OK) {
+    for (auto n : v) lb_ndt_destroy(n);
+    return st;
+  }
+  h->ndt = v;
+  return LB_OK;
+}
+
+// after registration_check and odometry_ndt_handles: applies the setting (params already validated)
+int odometry_set_registration(lb_odometry* h, int method, const lb_ndt_params* ndt) {
+  if (method == LB_REG_NDT)
+    for (auto n : h->ndt) LB_TRY(lb_ndt_set_params(n, ndt));
+  std::lock_guard<std::mutex> lk(h->mu);
+  h->method = method;
+  return LB_OK;
+}
+
 // the next ticket in submission order once it is done (mu not held); 1 = not done yet and block == 0
 int take_next(lb_odometry* h, int block, const char* who, Entry** out) {
   Entry* e = nullptr;
@@ -427,6 +516,7 @@ int lb_odometry_destroy(lb_odometry* h) {
   cudaSetDevice(h->device);
   for (auto& p : h->prep) if (p.cloud) { lb_cloud_release(p.cloud); p.cloud = nullptr; }
   for (auto g : h->gicp) lb_gicp_destroy(g);
+  for (auto n : h->ndt) lb_ndt_destroy(n);
   lb_voxel_destroy(h->vg);
   for (auto& s : h->ring) if (s.d) cudaFree(s.d);
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
@@ -472,6 +562,10 @@ int lb_odometry_set_normals(lb_odometry* h, int k, const float* viewpoint) {
   const float vp[3] = {viewpoint ? viewpoint[0] : 0.f, viewpoint ? viewpoint[1] : 0.f, viewpoint ? viewpoint[2] : 0.f};
   std::lock_guard<std::mutex> lk(h->mu);
   if (h->next_return != h->next_ticket) { set_error("lb_odometry_set_normals: pipeline not idle"); return LB_ERR_INVALID_ARG; }
+  if (k != 0 && h->method == LB_REG_NDT && !h->chain) {
+    set_error("lb_odometry_set_normals: the normals stage has no consumer under NDT registration");
+    return LB_ERR_UNSUPPORTED;
+  }
   if (h->next_ticket != 0 && (k != h->normals_k || memcmp(vp, h->normals_vp, sizeof(vp)) != 0)) {
     // the previous scan's prepared cloud was built with the old setting
     set_error("lb_odometry_set_normals: change before the first scan is submitted");
@@ -480,6 +574,13 @@ int lb_odometry_set_normals(lb_odometry* h, int k, const float* viewpoint) {
   h->normals_k = k;
   memcpy(h->normals_vp, vp, sizeof(vp));
   return LB_OK;
+}
+
+int lb_odometry_set_registration(lb_odometry* h, int method, const lb_ndt_params* ndt) {
+  if (!h) { set_error("lb_odometry_set_registration: null handle"); return LB_ERR_INVALID_ARG; }
+  LB_TRY(registration_check(h, method, ndt, "lb_odometry_set_registration"));
+  if (method == LB_REG_NDT) LB_TRY(odometry_ndt_handles(h));
+  return odometry_set_registration(h, method, ndt);
 }
 
 }  // extern "C"
@@ -586,6 +687,7 @@ int lb_odometry_launch_count(lb_odometry* h, uint64_t* n) {
   uint64_t tot = 0, v = 0;
   lb_voxel_launch_count(h->vg, &v); tot += v;
   for (auto g : h->gicp) { lb_gicp_launch_count(g, &v); tot += v; }
+  for (auto nd : h->ndt) { lb_ndt_launch_count(nd, &v); tot += v; }
   *n = tot;
   return LB_OK;
 }
@@ -595,8 +697,10 @@ int lb_odometry_launch_count(lb_odometry* h, uint64_t* n) {
 // ================================================================ lb_locus_*: the whole lidar callback
 // The core above with stage L behind stage G.  Per ticket, in order, stage L adopts the scan's prepared cloud as the
 // source of its own lb_gicp handle, aligns it against the caller's rolling submap and does the pose bookkeeping and map
-// updates of Locus.cc:462-543 (lo_pose.h).  It is the one stage that depends on the previous scan's result, so it is the
-// only serial one; V and G fill and register the following scans meanwhile.
+// updates of Locus.cc:462-543 (lo_pose.h).  With localization_method = NDT the align is that of stage L's lb_ndt handle
+// (source = the scan's filtered points in its ring slot, target = the submap's points); the GICP handle then only
+// transforms keyframes and, with the ICP covariance on, searches the map.  It is the one stage that depends on the
+// previous scan's result, so it is the only serial one; V and G fill and register the following scans meanwhile.
 #if !defined(LB_ODOMETRY_STUB) || defined(LB_LOCUS_STUB)
 
 namespace lb {
@@ -606,6 +710,7 @@ int submap_device(const lb_submap* m);
 struct lb_locus {
   lb_odometry* core = nullptr;
   lb_gicp* g = nullptr;            // stage L's handle (own stream); source = the shared cloud, target = the submap
+  lb_ndt* ndt = nullptr;           // stage L's NDT handle (own stream), created when localization NDT is first selected
   lb_submap* map = nullptr;        // the caller's
   float* d_xyz = nullptr;          // a keyframe's points in the fixed frame, max_points x 6 floats (xyz, normal)
   lb_locus_params P{};
@@ -639,15 +744,27 @@ int locus_insert(lb_locus* c, size_t n, lb_locus_result& r) {
 }
 
 // MotionUpdate(I) + MeasurementUpdate against the submap + the keyframe branch (PointCloudLocalization.cc:313-382,
-// Locus.cc:514-543)
-int locus_localize(lb_locus* c, const lo::Pose& I, size_t n, lb_locus_result& r) {
+// Locus.cc:514-543).  s: the scan's ring slot (its filtered points, the NDT source)
+int locus_localize(lb_locus* c, const lo::Pose& I, const Slot& s, lb_locus_result& r) {
+  const size_t n = s.n;
   const lo::Pose P = lo::update(c->L, I);
   float guess[16];
   lo::to_mat(P, guess);
-  LB_TRY(lb_gicp_set_target_submap(c->g, c->map));
-  LB_TRY(lb_gicp_align(c->g, guess, &r.localization));
+  const bool ndt = c->P.localization_method == LB_REG_NDT;
+  if (ndt) {
+    LB_TRY(lb_ndt_set_source(c->ndt, s.d, s.n, s.point_step, (size_t)s.xyz_off, LB_MEM_DEVICE));
+    LB_TRY(lb_ndt_set_target_submap(c->ndt, c->map));      // no device work while the map is unchanged
+    LB_TRY(lb_ndt_align(c->ndt, guess, &r.localization_ndt));
+    ndt_as_gicp(r.localization_ndt, r.localization);
+  } else {
+    LB_TRY(lb_gicp_set_target_submap(c->g, c->map));
+    LB_TRY(lb_gicp_align(c->g, guess, &r.localization));
+  }
   r.has_localization = 1;
   if (c->P.icp_covariance.enabled) {
+    // PointCloudLocalization.cc:325-336 searches getSearchMethodTarget(), the target's kd-tree, for NDT too: the GICP
+    // handle takes the map as target for the 1-NN (the GICP align has done so already)
+    if (ndt) LB_TRY(lb_gicp_set_target_submap(c->g, c->map));
     // PointCloudLocalization.cc:325-336,398-421: the ICP covariance of this align, before the map changes.  The
     // reference's target is the mapper's neighbours in the frame of P (the align's guess); the submap is in the fixed
     // frame, so its normals are rotated by P^-1 (unpinned, DESIGN.md 4i)
@@ -690,6 +807,8 @@ void locus_scan(lb_locus* c, Entry* e) {
   memcpy(r.error, o.error, sizeof(r.error));
   r.has_odometry = o.has_pose;
   r.odometry = o.gicp;
+  r.odometry_ndt = o.ndt;
+  const Slot& slot = c->core->ring[o.ticket % c->core->ring.size()];   // kept until this ticket is done (voxel_stage)
   lb_cloud* cl = e->loc_cloud;
   e->loc_cloud = nullptr;
   lo::Pose I = lo::identity();
@@ -709,9 +828,9 @@ void locus_scan(lb_locus* c, Entry* e) {
         // Locus.cc:462-472: the first scan seeds the map at the initial pose -- unless a prior map is loaded, in
         // which case it is localized against it like any other scan (with I = identity)
         c->started = true;
-        st = c->P.prior_map ? locus_localize(c, I, o.n_filtered, r) : locus_insert(c, o.n_filtered, r);
+        st = c->P.prior_map ? locus_localize(c, I, slot, r) : locus_insert(c, o.n_filtered, r);
       } else {
-        st = locus_localize(c, I, o.n_filtered, r);
+        st = locus_localize(c, I, slot, r);
       }
     }
     if (st != LB_OK) { r.status = st; copy_err(r.error, sizeof(r.error)); }
@@ -778,11 +897,44 @@ int locus_apply_params(lb_locus* c, const lb_locus_params* p) {
     set_error("lb_locus_set_params: icp_covariance.max_covariance must be finite and > 0");
     return LB_ERR_INVALID_ARG;
   }
+  // registration methods: checked (and their NDT handles made) before anything changes
+  LB_TRY(registration_check(c->core, p->odometry_method, &p->odometry_ndt, "lb_locus_set_params"));
+  if (p->localization_method != LB_REG_GICP && p->localization_method != LB_REG_NDT) {
+    set_error("lb_locus_set_params: localization_method must be LB_REG_GICP (0) or LB_REG_NDT (1)");
+    return LB_ERR_INVALID_ARG;
+  }
+  if (p->localization_method == LB_REG_NDT) LB_TRY(ndt_check_params(&p->localization_ndt, "lb_locus_set_params"));
+  bool submitted;
+  {
+    std::lock_guard<std::mutex> lk(c->core->mu);
+    submitted = c->core->next_ticket != 0;
+  }
+  if (submitted && p->localization_method != c->P.localization_method) {
+    set_error("lb_locus_set_params: change the registration method before the first scan is submitted");
+    return LB_ERR_UNSUPPORTED;
+  }
+  if (p->odometry_method == LB_REG_NDT) LB_TRY(odometry_ndt_handles(c->core));
+  if (p->localization_method == LB_REG_NDT && !c->ndt) {
+    lb_ndt* n = nullptr;
+    LB_TRY(lb_ndt_create(c->core->device, &n));
+    const int s = ndt_reserve(n, c->core->max_points);       // the scan side; the map side grows with the map
+    if (s != LB_OK) { lb_ndt_destroy(n); return s; }
+    c->ndt = n;
+  }
   LB_TRY(lb_odometry_set_normals(c->core, fe.normals_k, fe.viewpoint));
   int st = lb_gicp_set_params(c->g, &p->localization);
   if (st == LB_OK) {
     st = lb_odometry_set_gicp_params(c->core, &p->odometry);
     if (st != LB_OK) lb_gicp_set_params(c->g, &c->P.localization);   // keep the previous state
+  }
+  if (st == LB_OK) {
+    st = odometry_set_registration(c->core, p->odometry_method, &p->odometry_ndt);
+    if (st == LB_OK && p->localization_method == LB_REG_NDT) st = lb_ndt_set_params(c->ndt, &p->localization_ndt);
+    if (st != LB_OK) {
+      lb_gicp_set_params(c->g, &c->P.localization);
+      lb_odometry_set_gicp_params(c->core, &c->P.odometry);
+      odometry_set_registration(c->core, c->P.odometry_method, &c->P.odometry_ndt);
+    }
   }
   if (st != LB_OK) {
     lb_odometry_set_normals(c->core, c->P.front_end.normals_k, c->P.front_end.viewpoint);
@@ -835,6 +987,16 @@ int lb_locus_default_params(lb_locus_params* p) {
   for (int i = 0; i < 16; i++) p->initial_pose[i] = (i % 5 == 0) ? 1.0 : 0.0;
   p->icp_covariance.enabled = 0;               // off: the chain computes what it computed without it
   p->icp_covariance.max_covariance = 0.01;     // point_cloud_localization/config/parameters.yaml icp_max_covariance
+  // registration_method: gicp in both packages; their NDT settings (PointCloudOdometry.cc:182-195,
+  // PointCloudLocalization.cc:267-280) take the same icp_tf_epsilon / icp_iterations (tf_epsilon / iterations) values
+  p->odometry_method = LB_REG_GICP;
+  p->localization_method = LB_REG_GICP;
+  lb_ndt_default_params(&p->odometry_ndt);
+  p->odometry_ndt.transformation_epsilon = 0.001;
+  p->odometry_ndt.max_iterations = 20;
+  lb_ndt_default_params(&p->localization_ndt);
+  p->localization_ndt.transformation_epsilon = 0.00001;
+  p->localization_ndt.max_iterations = 20;
   return LB_OK;
 }
 
@@ -858,6 +1020,7 @@ int lb_locus_create(int device, int depth, size_t max_points, uint32_t max_point
   if (st == LB_OK) st = locus_apply_params(c, &P);
   if (st != LB_OK) {
     if (c->g) lb_gicp_destroy(c->g);
+    if (c->ndt) lb_ndt_destroy(c->ndt);
     if (c->core) lb_odometry_destroy(c->core);
     if (c->d_xyz) cudaFree(c->d_xyz);
     delete c;
@@ -878,6 +1041,7 @@ int lb_locus_destroy(lb_locus* c) {
   if (c->lthread.joinable()) c->lthread.join();
   cudaSetDevice(c->core->device);
   lb_gicp_destroy(c->g);
+  if (c->ndt) lb_ndt_destroy(c->ndt);
   lb_odometry_destroy(c->core);    // joins stages V and G, releases the clouds of the scans still in flight
   cudaFree(c->d_xyz);
   delete c;

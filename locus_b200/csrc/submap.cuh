@@ -57,6 +57,10 @@ int submap_target_normals(const lb_submap* m, uint64_t generation, const f4** nr
   *nrm = m->nrm_on ? m->nrm[m->cur].p : nullptr;
   return LB_OK;
 }
+// the map's current points for lb_ndt_set_target_submap (ndt.cu): float4 records (stride 16, w unused), insertion order
+void submap_points_view(const lb_submap* m, const f4** pts, size_t* n, uint64_t* generation, cudaStream_t* stream) {
+  *pts = m->pts[m->cur].p; *n = m->n; *generation = m->generation; *stream = m->eng->c.stream;
+}
 }  // namespace lb
 
 namespace {

@@ -184,6 +184,9 @@ class B200Ndt {
 
   bool setInputSource(const PointF* pts, size_t n) { return lb_ndt_set_source(h_, pts, n, sizeof(PointF), 0, LB_MEM_HOST) == LB_OK; }
   bool setInputTarget(const PointF* pts, size_t n) { return lb_ndt_set_target(h_, pts, n, sizeof(PointF), 0, LB_MEM_HOST) == LB_OK; }
+  // the resident submap's points as the target, gathered on the device; call again after the map changed (a no-op while
+  // it is unchanged)
+  bool setInputTargetSubmap(lb_submap* m) { return lb_ndt_set_target_submap(h_, m) == LB_OK; }
   bool align(const Matrix4f* guess = nullptr) { return lb_ndt_align(h_, guess ? guess->data() : nullptr, &r_) == LB_OK; }
   Matrix4f getFinalTransformation() const {
     Matrix4f m;
@@ -294,6 +297,13 @@ class B200Odometry {
   bool applyParams() { return lb_odometry_set_gicp_params(h_, &p_) == LB_OK; }
   // normals stage (k = 0: off): every filtered scan gets its k-NN normals; idle pipeline, before the first scan
   bool setNormals(int k, const float* viewpoint = nullptr) { return lb_odometry_set_normals(h_, k, viewpoint) == LB_OK; }
+  // registration_method: LB_REG_GICP (default) or LB_REG_NDT with its params (nullptr = lb_ndt_default_params); idle
+  // pipeline, before the first scan
+  bool setRegistration(int method, const lb_ndt_params* ndt = nullptr) {
+    lb_ndt_params p;
+    if (ndt) p = *ndt; else lb_ndt_default_params(&p);
+    return lb_odometry_set_registration(h_, method, &p) == LB_OK;
+  }
 
   // scan (and filtered_out, if given) must stay valid until next() has returned this ticket
   bool submit(const uint8_t* scan, size_t n_pts, uint32_t point_step, const std::vector<lb_field>& fields,
@@ -337,6 +347,13 @@ class B200Locus {
   lb_locus_params& params() { return p_; }                      // edit, then applyParams() while nothing is in flight
   bool applyParams() { return lb_locus_set_params(h_, &p_) == LB_OK; }
   // params().front_end: normals and adaptive input voxelization (off by default; shipped values in locus_b200.h)
+  // params().odometry_method / localization_method (LB_REG_GICP or LB_REG_NDT) with odometry_ndt / localization_ndt:
+  // each package's registration_method; set before the first scan
+  bool setRegistration(int odometry_method, int localization_method) {
+    p_.odometry_method = odometry_method;
+    p_.localization_method = localization_method;
+    return applyParams();
+  }
 
   // scan (and filtered_out, if given) must stay valid until next() has returned this ticket
   bool submit(const uint8_t* scan, size_t n_pts, uint32_t point_step, const std::vector<lb_field>& fields,

@@ -36,6 +36,19 @@ the three clouds is part of stage V).  The line adds stage V busy ms per scan of
 VoxelGrid leaf (default here 0.5, which keeps the filtered scans within the SM budget of DESIGN.md 4i).
 
   python tools/bench_locus.py --lidars 3 --scans 60 --depth 3 --reps 3
+
+--odometry-method / --localization-method {gicp,ndt} set each package's registration_method in the default run (the
+other modes keep GICP): the chain arms register with lb_locus's NDT stages, the seq_* arms with blocking NdtB200 calls
+(the odometry against the previous filtered scan, the localization against the submap's points).
+
+  python tools/bench_locus.py --odometry-method ndt --localization-method ndt --scans 60 --depth 3 --reps 3
+
+--ndt-map-rebuild N times what an NDT localization pays after a keyframe: a submap of about N points (posed scans of the
+stream, 0.1 m map voxels), one point inserted (a new generation), then lb_ndt_set_target_submap plus the lazy build of the
+voxel Gaussians (through lb_ndt_target_voxels, which triggers it), host clock around the blocking calls, --reps x 10
+times; and the same call on the unchanged map.
+
+  python tools/bench_locus.py --ndt-map-rebuild 500000
 """
 import argparse
 import ctypes as C
@@ -74,6 +87,19 @@ def sequential(lb, blobs, d_blobs, prefill, params, device):
     odo, loc = lb.GicpB200(), lb.GicpB200()
     C.memmove(C.byref(odo._p), C.byref(P.odometry), C.sizeof(P.odometry)); odo._apply()
     C.memmove(C.byref(loc._p), C.byref(P.localization), C.sizeof(P.localization)); loc._apply()
+    odo_ndt, loc_ndt = P.odometry_method == lb.api.LB_REG_NDT, P.localization_method == lb.api.LB_REG_NDT
+    nodo, nloc = lb.NdtB200(), lb.NdtB200()
+    C.memmove(C.byref(nodo._p), C.byref(P.odometry_ndt), C.sizeof(P.odometry_ndt)); nodo._apply()
+    C.memmove(C.byref(nloc._p), C.byref(P.localization_ndt), C.sizeof(P.localization_ndt)); nloc._apply()
+
+    def ndt_cloud(h, which, src):
+        """an NDT source (which = 0) or target (1) from a host xyz array or a device filtered cloud (ptr, n, stride)"""
+        if src[1] is None:
+            (h.setInputSource if which == 0 else h.setInputTarget)(src[0])
+        else:
+            fn = lb.lib().lb_ndt_set_source if which == 0 else lb.lib().lb_ndt_set_target
+            lb.api._check(fn(h._h, C.c_void_p(src[0]), src[1], src[2], 0, lb.LB_MEM_DEVICE))
+
     m = lb.SubmapB200(0, MAP_RES)
     m.InsertPoints(prefill)
     n = blobs[0].size // STEP
@@ -95,14 +121,24 @@ def sequential(lb, blobs, d_blobs, prefill, params, device):
             src = (np.ascontiguousarray(f).view(np.float32).reshape(-1, 8)[:, :3].copy(), None, None)
             nf = src[0].shape[0]
         odoT = None
-        if prev is not None:
+        if prev is not None and odo_ndt:
+            ndt_cloud(nodo, 0, src); ndt_cloud(nodo, 1, prev)
+            nodo.align()
+            odoT = nodo.getFinalTransformation()
+        elif prev is not None:
             odo.setInputSource(*src); odo.setInputTarget(*prev)
             odo.align()
             odoT = odo.getFinalTransformation()
         loc.setInputSource(*src)
+        if loc_ndt:
+            ndt_cloud(nloc, 0, src)
         out = {}
 
         def localize(Gs):
+            if loc_ndt:
+                nloc.setTargetSubmap(m)
+                out["loc"] = nloc.align(Gs)
+                return nloc.getFinalTransformation()
             loc.setTargetSubmap(m)
             out["loc"] = loc.align(Gs)
             return loc.getFinalTransformation()
@@ -204,6 +240,41 @@ def pipelined(lb, blobs, d_blobs, prefill, params, device, depth, prefill_n=None
     ch.close()
     m.close()
     return dt, res, times
+
+
+def ndt_map_rebuild(lb, a, line):
+    """--ndt-map-rebuild: the submap's NDT target rebuilt after a change of the map, and the call on an unchanged map"""
+    scene, poses, _ = G.stream(a.seed, 2, a.beams, a.az)
+    m = lb.SubmapB200(0, MAP_RES)
+    k = 0
+    while m.size() < a.ndt_map_rebuild and k < 64:
+        # scans from poses around the origin, kept to LOCUS's 20 m window (box_filter_size) around it
+        T = G.pose_matrix([4.0 * (k % 7) - 12.0, 3.0 * (k // 7 % 7) - 9.0, 0.0], [0, 0, 0.4 * k])
+        w = G.world_points(scene, [T], a.seed + k, a.beams, a.az)
+        m.InsertPoints(np.ascontiguousarray(w[(np.abs(w) <= 20.0).all(axis=1)]))
+        k += 1
+    nd = lb.NdtB200()
+    L = lb.lib()
+    nv = C.c_size_t(0)
+
+    def target():
+        nd.setTargetSubmap(m)
+        lb.api._check(L.lb_ndt_target_voxels(nd._h, 0, C.byref(nv), None, None, None, None, None))
+
+    target()                                                  # modules, allocations
+    top = m.points().max(axis=0) - np.float32(0.5)            # free space inside the map's box: inserts land there
+    rebuild, unchanged = [], []
+    j = 0
+    for i in range(10 * a.reps):
+        while not m.InsertPoints((top - np.float32(0.13) * np.array([j % 50, j // 50, 0], np.float32)).reshape(1, 3)):
+            j += 1
+        j += 1
+        t0 = time.perf_counter(); target(); rebuild.append(time.perf_counter() - t0)
+        t0 = time.perf_counter(); target(); unchanged.append(time.perf_counter() - t0)
+    line.update(map_points=m.size(), window_half_size=20.0, map_resolution=MAP_RES, searchable_voxels=nv.value, ndt_resolution=nd.getResolution(),
+                rebuild_ms_median=1e3 * float(np.median(rebuild)), rebuild_ms_min=1e3 * float(np.min(rebuild)),
+                unchanged_ms_median=1e3 * float(np.median(unchanged)))
+    m.close()
 
 
 def merged_inputs(scans, mounts):
@@ -446,12 +517,22 @@ def main():
     ap.add_argument("--lidars", type=int, default=1, choices=(1, 3),
                     help="3: every scan is three lidars merged in the VoxelGrid stage (lb_locus_submit_merged)")
     ap.add_argument("--leaf", type=float, default=None, help="VoxelGrid leaf of --lidars 3 (default 0.5)")
+    ap.add_argument("--odometry-method", choices=("gicp", "ndt"), default="gicp", help="registration_method of the odometry")
+    ap.add_argument("--ndt-map-rebuild", type=int, default=0, metavar="N",
+                    help="time the NDT target of an N-point submap after a change of the map")
+    ap.add_argument("--localization-method", choices=("gicp", "ndt"), default="gicp",
+                    help="registration_method of the localization")
     a = ap.parse_args()
     if a.icp_covariance and "--reps" not in sys.argv:
         a.reps = 3
     import torch
     import locus_b200 as lb
     assert lb.device_count() > 0, "bench_locus needs a CUDA device"
+    if a.ndt_map_rebuild:
+        line = {"card": card()}
+        ndt_map_rebuild(lb, a, line)
+        emit(line, a.out)
+        return
     if a.lidars == 3:
         line = {"scans": a.scans, "depth": a.depth, "card": card(), "arms": {}}
         lidars(lb, a, line)
@@ -461,7 +542,8 @@ def main():
     world = G.world_points(scene, [poses[0], G.pose_matrix([1.0, 0.5, 0.0], [0, 0, 0.3])], a.seed, a.beams, a.az)
     vg = lb.VoxelGridB200(); vg.setLeafSize(0.2)
     prefill = np.ascontiguousarray(vg.filter(G.xyz_blob(world), STEP, lb.xyzi_fields())).view(np.float32).reshape(-1, 8)[:, :3].copy()
-    params = dict(translation_threshold_kf=0.6, refresh_every=2)
+    params = dict(translation_threshold_kf=0.6, refresh_every=2, odometry_method=a.odometry_method,
+                  localization_method=a.localization_method)
     line = {"scans": a.scans, "raw_points_per_scan": blobs[0].size // STEP, "depth": a.depth, "card": card(),
             "params": dict(params, leaf=LEAF, map_resolution=MAP_RES), "arms": {}}
     if a.front_end:
